@@ -1,19 +1,17 @@
-// r3g_attention: O = softmax(Q K^T * scale) V for head_dim 64, no mask -- flash-attention forward on tcgen05.
+// r3g_attention: O = softmax(Q K^T * scale) V for head_dim 64, no mask -- flash-attention forward on wgmma (sm_90a).
 //
-// One CTA = one 128-row query tile of one (batch, head); two CTAs are co-resident per SM so that one CTA's
-// softmax (exp-unit bound at head_dim 64) overlaps the other's MMAs.
-//   warps 0..3  softmax / lazy correction / epilogue: thread t owns query row t (TMEM lane t): row max and row
-//               sum need no shuffles; P goes back to TMEM as packed fp16 and is the A operand of P V
-//   warp 4      TMA producer: Q once, then K and V tiles (128 x 64) through 2-deep rings
-//   warp 5      MMA issuer:  S = Q K^T  (M128 N128 K16 x4, accumulator in TMEM)
-//                            O += P V   (M128 N64  K16 x8, A from TMEM, V consumed MN-major from its row-major tile)
+// One CTA = one 192-row query tile of one (batch, head):
+//   warps 0..11  three consumer warpgroups, 64 query rows each.  Per 128-key tile: S = Q K^T (wgmma m64n128k16 x4,
+//                both operands from shared memory, fp32 accumulators in registers); online softmax in registers (a
+//                row lives in the 4 threads of a quad: two shuffles for its max); P is packed to fp16 in registers and
+//                is directly the A operand of O += P V (wgmma m64n64k16 x8, V read MN-major from its row-major tile).
+//   warp 12      TMA producer: Q once, then K and V tiles (128 x 64) through 3-deep rings.
+// Three warpgroups per SM let one warpgroup's softmax overlap the others' MMAs.
 // Call sites replaced: F.scaled_dot_product_attention in hunyuan3ddit.py:33-36 (L = 4442 joint txt+img tokens),
 // attention_blocks.py:328 (ShapeVAE, L = 3072), attention_processors.py:29-32 (geo-decoder cross attention,
-// Lk = 3072), vggt/layers/attention.py:61.  Earlier kernel generations (registers-accumulated O, two threads per
-// row) live in the git history (round 1) with their measurements in profiles/README.md.
+// Lk = 3072), vggt/layers/attention.py:61.
 #include <cuda_fp16.h>
 #include <math.h>
-#include <stdlib.h>
 
 #include "r3g_internal.h"
 #include "r3g_ptx.cuh"
@@ -23,15 +21,15 @@ namespace {
 using namespace r3g;
 
 constexpr int kD = 64;
-constexpr int kBQ = 128;
+constexpr int kWG = 3;                            // consumer warpgroups
+constexpr int kBQ = 64 * kWG;                     // query rows per CTA
 constexpr int kBKV = 128;
-constexpr int kKVStages = 2;
-constexpr int kTileBytes = 128 * kD * 2;          // 16 KB: Q, K and V tiles
-constexpr int kPBytes = kBQ * kBKV * 2;           // 32 KB
-constexpr int kTilesBytes = kTileBytes * (1 + 2 * kKVStages) + kPBytes;  // 112 KB
-constexpr int kSmemBytes = kTilesBytes + 1024;    // + alignment slack, which also hosts the barriers
-constexpr uint32_t kTmemCols = 256;               // S: 128 columns, O_j: 64 columns
-constexpr uint32_t kTmemS = 0, kTmemO = 128;
+constexpr int kStg = 3;                           // K / V ring depth
+constexpr int kQBytes = 64 * kD * 2;              // 8 KB per warpgroup
+constexpr int kTileBytes = kBKV * kD * 2;         // 16 KB: K and V tiles
+constexpr int kTilesBytes = kQBytes * kWG + 2 * kStg * kTileBytes;   // 120 KB
+constexpr int kSmemBytes = kTilesBytes + 1024 + 256;   // + alignment slack + barriers
+constexpr int kThreads = 128 * kWG + 32;
 
 struct AttnParams {
   __half* o;
@@ -46,122 +44,19 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Software pipeline:
-//   * the whole S row (128 fp32) is pulled into registers in one go, the TMEM S buffer is released at once
-//     (s_free) so the MMA warp issues S_{j+1} = Q K_{j+1}^T BEFORE P_j V_j: the tensor pipe works on the next
-//     scores while this tile's softmax runs;
-//   * O accumulates in TMEM across tiles (tcgen05.mma accumulate); the running-max rescale is LAZY: rows are
-//     rescaled (TMEM load-multiply-store) only when the max grew by more than 2^8, so probabilities are bounded by
-//     256 (exact in the final normalisation, fp16-safe) and the common path never touches O;
-//   * exp2 on packed halves (ex2.approx.f16x2: two results per MUFU op, output already the fp16 P operand),
-//     3-input max, row sums accumulated as half2 partials and folded into fp32 every 16 columns.
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-__device__ __forceinline__ uint32_t cvt_f16x2(float lo, float hi) {
-  uint32_t d;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
-  return d;
-}
-__device__ __forceinline__ uint32_t ex2_f16x2(uint32_t x) {
-  uint32_t d;
-  asm("ex2.approx.f16x2 %0, %1;" : "=r"(d) : "r"(x));
-  return d;
-}
-__device__ __forceinline__ uint32_t hadd2_u32(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("add.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};\n" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-
-// 2^x on the FMA pipe: Cody-Waite split with the 1.5*2^23 rounding constant, cubic for 2^f on [-0.5, 0.5]
-// (max relative error 1.0e-4 < fp16 rounding), exponent re-inserted with one integer multiply-add.
-// 1 ALU + 6 FMA-pipe instructions instead of one MUFU.EX2: the exp unit (16 lanes/clk/SM) is what bounds this kernel.
-__device__ __forceinline__ float exp2_poly(float x) {
-  x = fmaxf(x, -30.f);                                   // masked columns (-inf) -> 2^-30 -> 0 in fp16
-  const float t = x + 12582912.f;                        // integer part lands in the low mantissa bits
-  const float f = x - (t - 12582912.f);
-  float pl = fmaf(0.0550081f, f, 0.24220917f);
-  pl = fmaf(pl, f, 0.69328282f);
-  pl = fmaf(pl, f, 1.0f);
-  return __int_as_float(__float_as_int(t) * 8388608 + __float_as_int(pl));   // (bits(t) << 23) + bits(p)
-}
-// Blackwell's packed fp32 pipe (FADD2 / FMUL2 / FFMA2: two IEEE fp32 operations per issued instruction, operands in
-// aligned 64-bit register pairs -- the S row arrives from tcgen05.ld already laid out that way).
-// exp2_poly on a pair: 2 FMNMX + 3 FADD2 + 3 FFMA2 + 2 IMAD for two results
-__device__ __forceinline__ void exp2_poly2(float x0, float x1, float& e0, float& e1) {
-  const uint64_t x = f2_pack(fmaxf(x0, -30.f), fmaxf(x1, -30.f));
-  const uint64_t magic = f2_pack(12582912.f, 12582912.f), nmagic = f2_pack(-12582912.f, -12582912.f);
-  const uint64_t t = f2_add(x, magic);
-  const uint64_t ti = f2_add(t, nmagic);
-  float i0, i1;
-  f2_unpack(ti, i0, i1);
-  const uint64_t f = f2_add(x, f2_pack(-i0, -i1));
-  uint64_t pl = f2_fma(f2_pack(0.0550081f, 0.0550081f), f, f2_pack(0.24220917f, 0.24220917f));
-  pl = f2_fma(pl, f, f2_pack(0.69328282f, 0.69328282f));
-  pl = f2_fma(pl, f, f2_pack(1.0f, 1.0f));
-  float t0, t1, p0, p1;
-  f2_unpack(t, t0, t1);
-  f2_unpack(pl, p0, p1);
-  e0 = __int_as_float(__float_as_int(t0) * 8388608 + __float_as_int(p0));
-  e1 = __int_as_float(__float_as_int(t1) * 8388608 + __float_as_int(p1));
-}
-
-constexpr float kRescaleThreshold = 8.f;  // log2 units
-
-constexpr int kThreadsV2 = 192;
-
-// kStg: K/V pipeline depth (3 only with kPT: the P tile's 32 KB of shared memory hold the third stage)
-// kF2: scale-and-subtract and the polynomial exponentials on the packed fp32 pipe (FFMA2 / FADD2)
-template <bool kPT, bool kF32, int kPoly, int kStg, bool kF2 = false>
-__global__ void __launch_bounds__(kThreadsV2, 2)
+__global__ void __launch_bounds__(kThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const uintptr_t raw = reinterpret_cast<uintptr_t>(smem_raw);
-  const uintptr_t aligned = (raw + 1023) & ~(uintptr_t)1023;
-  uint8_t* smem = reinterpret_cast<uint8_t*>(aligned);
-  uint8_t* bar_mem = (aligned - raw >= 256) ? smem_raw : smem + kTilesBytes;
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + kTileBytes;
+  uint8_t* sK = sQ + kWG * kQBytes;
   uint8_t* sV = sK + kStg * kTileBytes;
-  uint8_t* sP = sV + kStg * kTileBytes;
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(bar_mem);
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + kTilesBytes);
   uint64_t* k_full = q_full + 1;
   uint64_t* v_full = k_full + kStg;
   uint64_t* k_empty = v_full + kStg;
   uint64_t* v_empty = k_empty + kStg;
-  uint64_t* s_full = v_empty + kStg;
-  uint64_t* s_free = s_full + 1;
-  uint64_t* p_full = s_free + 1;
-  uint64_t* o_full = p_full + 1;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(o_full + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -169,7 +64,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int h = blockIdx.y, b = blockIdx.z;
   const int n_kv = (p.Lk + kBKV - 1) / kBKV;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 4 * kWG && lane == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
@@ -177,27 +72,22 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     for (int s = 0; s < kStg; ++s) {
       mbar_init(&k_full[s], 1);
       mbar_init(&v_full[s], 1);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&v_empty[s], 1);
+      mbar_init(&k_empty[s], 128 * kWG);
+      mbar_init(&v_empty[s], 128 * kWG);
     }
-    mbar_init(s_full, 1);
-    mbar_init(s_free, 128);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<kTmemCols>(tmem_base_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   pdl_wait();      // q / k / v come from the projection kernel before us (no trigger here: a multi-wave grid must not
                    // let the next kernel's CTAs take SM slots from its own later waves; the implicit one at exit is used)
 
-  if (warp == 4) {
+  if (warp == 4 * kWG) {
+    // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      mbar_expect_tx(q_full, kTileBytes);
-      tma_load_4d(sQ, &tmap_q, q_full, 0, q0, h, b, kEvictFirst);
+      // a warpgroup whose 64 rows all lie past Lq gets no Q (it computes on stale data and stores nothing)
+      const int groups = min(kWG, (p.Lq - q0 + 63) / 64);
+      mbar_expect_tx(q_full, groups * kQBytes);
+      for (int g = 0; g < groups; ++g) tma_load_4d(sQ + g * kQBytes, &tmap_q, q_full, 0, q0 + 64 * g, h, b, kEvictFirst);
       for (int j = 0; j < n_kv; ++j) {
         const int st = j % kStg;
         const uint32_t ph = (j / kStg) & 1;
@@ -209,220 +99,103 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         tma_load_4d(sV + st * kTileBytes, &tmap_v, &v_full[st], 0, j * kBKV, h, b, kEvictLast);
       }
     }
-  } else if (warp == 5) {
-    constexpr uint32_t idesc_s = umma_idesc_f16(kBQ, kBKV, false, false);
-    constexpr uint32_t idesc_o = umma_idesc_f16(kBQ, kD, false, true);
-    const uint32_t aq = smem_u32(sQ);
-    auto issue_s = [&](int j) {
-      const int st = j % kStg;
-      mbar_wait(&k_full[st], (j / kStg) & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t ak = smem_u32(sK + st * kTileBytes);
-#pragma unroll
-        for (int k = 0; k < kD / 16; ++k)
-          umma_ss(tmem_base + kTmemS, umma_desc_sw128(aq + k * 32, 1024, 16), umma_desc_sw128(ak + k * 32, 1024, 16),
-                  idesc_s, k ? 1u : 0u);
-        umma_commit(s_full);
-        umma_commit(&k_empty[st]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(q_full, 0);
-    issue_s(0);
-    for (int j = 0; j < n_kv; ++j) {
-      if (j + 1 < n_kv) {
-        mbar_wait(s_free, j & 1);  // S_j now lives in the softmax warps' registers
-        issue_s(j + 1);
-      }
-      const int st = j % kStg;
-      mbar_wait(p_full, j & 1);
-      mbar_wait(&v_full[st], (j / kStg) & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t ap = smem_u32(sP), av = smem_u32(sV + st * kTileBytes);
-#pragma unroll
-        for (int k = 0; k < kBKV / 16; ++k) {
-          if (kPT)
-            umma_ts(tmem_base + kTmemO, tmem_base + 192 + k * 8, umma_desc_sw128(av + k * 2048, 1024, 1024), idesc_o,
-                    (j | k) ? 1u : 0u);
-          else
-            umma_ss(tmem_base + kTmemO, umma_desc_sw128(ap + (k >> 2) * (kBQ * 128) + (k & 3) * 32, 1024, 16),
-                    umma_desc_sw128(av + k * 2048, 1024, 1024), idesc_o, (j | k) ? 1u : 0u);
-        }
-        umma_commit(o_full);
-        umma_commit(&v_empty[st]);
-      }
-      __syncwarp();
-    }
-  } else if (warp < 4) {
-    const int row = threadIdx.x;
-    const uint32_t lane_base = (uint32_t)(warp * 32);
-    float m_used = -INFINITY, l_run = 0.f;
-    const uint32_t p_row = smem_u32(sP) + (row >> 3) * 1024 + (row & 7) * 128;
-    const int sw = row & 7;
-    for (int j = 0; j < n_kv; ++j) {
-      const int valid = min(kBKV, p.Lk - j * kBKV);
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      uint32_t s[kBKV];
-#pragma unroll
-      for (int c = 0; c < kBKV; c += 32) tmem_ld32(tmem_addr(tmem_base, lane_base, kTmemS + c), &s[c]);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(s_free);
-      if (valid < kBKV) {
-#pragma unroll
-        for (int i = 0; i < kBKV; ++i)
-          if (i >= valid) s[i] = 0xff800000u;  // -inf
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;   // four chains: the 3-input max
-#pragma unroll                                                                   // has a 4-cycle dependent latency
-      for (int i = 0; i < kBKV; i += 8) {
-        mx0 = fmax3(mx0, __uint_as_float(s[i]), __uint_as_float(s[i + 1]));
-        mx1 = fmax3(mx1, __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]));
-        mx2 = fmax3(mx2, __uint_as_float(s[i + 4]), __uint_as_float(s[i + 5]));
-        mx3 = fmax3(mx3, __uint_as_float(s[i + 6]), __uint_as_float(s[i + 7]));
-      }
-      const float m_new = fmaxf(fmax3(mx0, mx1, mx2), mx3) * p.scale_log2;
-      bool waited_o = (j == 0);
-      if (j == 0) {
-        m_used = m_new;
-      } else {
-        const bool need = m_new - m_used > kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {
-          // rare: the O accumulator must be rescaled; P_{j-1} V_{j-1} has to have completed first
-          mbar_wait(o_full, (j - 1) & 1);
-          tc_fence_after();
-          waited_o = true;
-          const float alpha = need ? ex2(m_used - m_new) : 1.f;
-#pragma unroll 1
-          for (int c = 0; c < kD; c += 8) {   // 8 columns at a time keeps the S row in registers
-            uint32_t o[8];
-            tmem_ld8(tmem_addr(tmem_base, lane_base, kTmemO + c), o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 8; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st8(tmem_addr(tmem_base, lane_base, kTmemO + c), o);
-          }
-          tmem_st_wait();
-          l_run *= alpha;
-          if (need) m_used = m_new;
-        }
-      }
-      // probabilities for the whole row first (registers: the packed P row reuses the S row's registers) ...
-      float rs = 0.f;
-      uint32_t carry = 0;
-      const uint64_t scale2 = f2_pack(p.scale_log2, p.scale_log2), nm2 = f2_pack(-m_used, -m_used);
-      uint32_t pk[kBKV / 2];
-#pragma unroll
-      for (int c = 0; c < kBKV; c += 16) {
-#pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-          float x0, x1;
-          if (kF2) {
-            f2_unpack(f2_fma(f2_pack(__uint_as_float(s[c + i]), __uint_as_float(s[c + i + 1])), scale2, nm2), x0, x1);
-          } else {
-            x0 = fmaf(__uint_as_float(s[c + i]), p.scale_log2, -m_used);
-            x1 = fmaf(__uint_as_float(s[c + i + 1]), p.scale_log2, -m_used);
-          }
-          if (kPoly > 0 && (((c + i) >> 1) % (kPoly > 0 ? kPoly : 1)) == kPoly - 1) {
-            if (kF2) {
-              float e0, e1;
-              exp2_poly2(x0, x1, e0, e1);
-              pk[(c + i) >> 1] = cvt_f16x2(e0, e1);
-            } else {
-              pk[(c + i) >> 1] = cvt_f16x2(exp2_poly(x0), exp2_poly(x1));
-            }
-          } else {
-            pk[(c + i) >> 1] = kF32 ? cvt_f16x2(ex2(x0), ex2(x1)) : ex2_f16x2(cvt_f16x2(x0, x1));
-          }
-        }
-        const uint32_t* q8 = &pk[c >> 1];
-        const uint32_t a01 = hadd2_u32(hadd2_u32(q8[0], q8[1]), hadd2_u32(q8[2], q8[3]));
-        const uint32_t a23 = hadd2_u32(hadd2_u32(q8[4], q8[5]), hadd2_u32(q8[6], q8[7]));
-        if (kF32) {
-          // 16 packed pairs (32 probabilities <= 1, partial sums <= 16) summed as half2 before the fp32 accumulate
-          const uint32_t a16 = hadd2_u32(a01, a23);
-          if ((c & 16) == 0) {
-            carry = a16;
-          } else {
-            const uint32_t a32 = hadd2_u32(carry, a16);
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&a32));
-            rs += f.x + f.y;
-          }
-        } else {
-          const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&a01));
-          const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&a23));
-          rs += (f0.x + f0.y) + (f1.x + f1.y);
-        }
-      }
-      // ... and only then wait for the previous P V to release the P tile: the exponentials above ran under it
-      if (!waited_o) {
-        mbar_wait(o_full, (j - 1) & 1);
-        tc_fence_after();
-      }
-      if (kPT) {
-        tmem_st32(tmem_addr(tmem_base, lane_base, 192), &pk[0]);
-        tmem_st32(tmem_addr(tmem_base, lane_base, 224), &pk[32]);
-        tmem_st_wait();
-      } else {
-#pragma unroll
-        for (int c = 0; c < kBKV; c += 8) {
-          const uint32_t addr = p_row + (c >> 6) * (kBQ * 128) + (((((c & 63) >> 3)) ^ sw) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(pk[(c >> 1)]),
-                       "r"(pk[(c >> 1) + 1]), "r"(pk[(c >> 1) + 2]), "r"(pk[(c >> 1) + 3])
-                       : "memory");
-        }
-        fence_proxy_async_smem();
-      }
-      l_run += rs;
-      tc_fence_before();
-      mbar_arrive(p_full);
-    }
-    mbar_wait(o_full, (n_kv - 1) & 1);
-    tc_fence_after();
-    const float inv_l = 1.f / l_run;
-    const int qrow = q0 + row;
-    __half* op = p.o + (int64_t)b * p.o_sb + (int64_t)h * p.o_sh + (int64_t)qrow * p.o_sl;
-#pragma unroll
-    for (int c = 0; c < kD; c += 32) {
-      uint32_t v[32];
-      tmem_ld32(tmem_addr(tmem_base, lane_base, kTmemO + c), v);
-      tmem_ld_wait();
-      if (qrow < p.Lq) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 o4;
-          uint32_t* ow = reinterpret_cast<uint32_t*>(&o4);
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            ow[i] = pack_half2(__uint_as_float(v[8 * q + 2 * i]) * inv_l, __uint_as_float(v[8 * q + 2 * i + 1]) * inv_l);
-          *reinterpret_cast<uint4*>(op + c + 8 * q) = o4;
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
+  // -------------------------------------------------------------------- consumers
+  // accumulator layout (r3g_ptx.cuh): element i of a thread is row r0 + 8 ((i / 2) % 2), column 8 (i / 4) + c0 + i % 2
+  const int wg = warp >> 2;
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  const uint32_t aq = smem_u32(sQ + wg * kQBytes);
+  float o[kD / 2];
+#pragma unroll
+  for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int st = j % kStg;
+    const uint32_t ph = (j / kStg) & 1;
+    float s[kBKV / 2];
+    mbar_wait(&k_full[st], ph);
+    const uint32_t ak = smem_u32(sK + st * kTileBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kD / 16; ++k)
+      wgmma_m64n128k16_ss(s, gmma_desc_sw128(aq + k * 32, 1024, 16), gmma_desc_sw128(ak + k * 32, 1024, 16),
+                          k ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence<kBKV / 2>(s);
+    mbar_arrive(&k_empty[st]);
+
+    const int valid = min(kBKV, p.Lk - j * kBKV);
+    if (valid < kBKV) {
+#pragma unroll
+      for (int i = 0; i < kBKV / 2; ++i)
+        if (8 * (i >> 2) + c0 + (i & 1) >= valid) s[i] = -INFINITY;
+    }
+    // row maxima (rows r0 and r0 + 8) over the quad, in log2 units
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < kBKV / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    float alpha[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
+      mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 2));
+      const float m_new = fmaxf(m_run[rr], mx[rr] * p.scale_log2);
+      alpha[rr] = ex2(m_run[rr] - m_new);   // 0 on the first tile (m_run = -inf)
+      m_run[rr] = m_new;
+      l_run[rr] *= alpha[rr];
+    }
+#pragma unroll
+    for (int i = 0; i < kD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    // probabilities, packed to fp16 in the A-operand layout of the P V MMA (16 keys per k-step)
+    uint32_t pk[kBKV / 16][4];
+#pragma unroll
+    for (int i = 0; i < kBKV / 2; i += 2) {
+      const int rr = (i >> 1) & 1;
+      const float e0 = ex2(fmaf(s[i], p.scale_log2, -m_run[rr]));
+      const float e1 = ex2(fmaf(s[i + 1], p.scale_log2, -m_run[rr]));
+      l_run[rr] += e0 + e1;
+      pk[i >> 3][(i >> 1) & 3] = pack_half2(e0, e1);
+    }
+    mbar_wait(&v_full[st], ph);
+    const uint32_t av = smem_u32(sV + st * kTileBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBKV / 16; ++k) wgmma_m64n64k16_rs_tb(o, pk[k], gmma_desc_sw128(av + k * 2048, 1024, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence<kD / 2>(o);
+    mbar_arrive(&v_empty[st]);
+  }
+
+  float inv_l[2];
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    float l = l_run[rr];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv_l[rr] = 1.f / l;
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int qrow = q0 + wg * 64 + r0 + 8 * rr;
+    if (qrow >= p.Lq) continue;
+    __half* op = p.o + (int64_t)b * p.o_sb + (int64_t)h * p.o_sh + (int64_t)qrow * p.o_sl;
+#pragma unroll
+    for (int i = 2 * rr; i < kD / 2; i += 4)
+      *reinterpret_cast<uint32_t*>(op + 8 * (i >> 2) + c0) = pack_half2(o[i] * inv_l[rr], o[i + 1] * inv_l[rr]);
   }
 }
 
-
-using AttnKernel = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnParams);
-// the shipped specialisation: P in TMEM, scalar f32 exponentials, every 4th pair polynomial, 2-deep K/V rings,
-// packed-fp32 softmax arithmetic (the sweep over the other combinations is recorded in profiles/README.md)
-const AttnKernel kAttention = attention_kernel<true, true, 4, 2, true>;
-
 int make_qkv_map(r3g_ctx* ctx, CUtensorMap* m, const void* base, int64_t sb, int64_t sh, int64_t sl, int B, int H,
-                 int L) {
+                 int L, int box_rows) {
   const uint64_t dims[4] = {(uint64_t)kD, (uint64_t)L, (uint64_t)H, (uint64_t)B};
   const uint64_t strides[4] = {2, (uint64_t)sl * 2, (uint64_t)sh * 2, (uint64_t)sb * 2};
-  const uint32_t box[4] = {(uint32_t)kD, 128, 1, 1};
+  const uint32_t box[4] = {(uint32_t)kD, (uint32_t)box_rows, 1, 1};
   return r3g_make_tmap_f16(ctx, m, base, 4, dims, strides, box);
 }
 
@@ -438,21 +211,21 @@ extern "C" int r3g_attention(r3g_ctx* ctx, const r3g_attention_args* a, void* st
     return r3g_fail(ctx, R3G_E_INVALID, "attention: output strides must be multiples of 8 halfs");
   CUtensorMap mq, mk, mv;
   int rc;
-  if ((rc = make_qkv_map(ctx, &mq, a->q, a->q_sb, a->q_sh, a->q_sl, a->B, a->H, a->Lq))) return rc;
-  if ((rc = make_qkv_map(ctx, &mk, a->k, a->k_sb, a->k_sh, a->k_sl, a->B, a->H, a->Lk))) return rc;
-  if ((rc = make_qkv_map(ctx, &mv, a->v, a->v_sb, a->v_sh, a->v_sl, a->B, a->H, a->Lk))) return rc;
+  if ((rc = make_qkv_map(ctx, &mq, a->q, a->q_sb, a->q_sh, a->q_sl, a->B, a->H, a->Lq, 64))) return rc;
+  if ((rc = make_qkv_map(ctx, &mk, a->k, a->k_sb, a->k_sh, a->k_sl, a->B, a->H, a->Lk, kBKV))) return rc;
+  if ((rc = make_qkv_map(ctx, &mv, a->v, a->v_sb, a->v_sh, a->v_sl, a->B, a->H, a->Lk, kBKV))) return rc;
   AttnParams p;
   p.o = (__half*)a->o;
   p.o_sb = a->o_sb; p.o_sh = a->o_sh; p.o_sl = a->o_sl;
   p.Lq = a->Lq; p.Lk = a->Lk;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   if (!(ctx->attr_done & R3G_ATTR_ATTENTION)) {   // function attributes are per device: one flag per context
-    R3G_CUDA_OK(ctx, cudaFuncSetAttribute(kAttention, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    R3G_CUDA_OK(ctx, cudaFuncSetAttribute(kAttention, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    R3G_CUDA_OK(ctx, cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    R3G_CUDA_OK(ctx, cudaFuncSetAttribute(attention_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     ctx->attr_done |= R3G_ATTR_ATTENTION;
   }
   dim3 grid((a->Lq + kBQ - 1) / kBQ, a->H, a->B);
-  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, kAttention, grid, dim3(kThreadsV2), kSmemBytes, (cudaStream_t)stream, mq, mk, mv, p));
+  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, attention_kernel, grid, dim3(kThreads), kSmemBytes, (cudaStream_t)stream, mq, mk, mv, p));
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;
 }

@@ -1,5 +1,5 @@
 // Convolution support for VGGT's DPT depth head (vggt/vggt/heads/dpt_head.py:172-291): every convolution runs as a
-// GEMM on the tcgen05 linear kernel over channels-last (NHWC) fp16 feature maps --
+// GEMM on the wgmma linear kernel (gemm.cu) over channels-last (NHWC) fp16 feature maps --
 //   1x1 convolution, ConvTranspose2d with kernel == stride : r3g_linear directly on the [N*H*W, C] rows,
 //   3x3 convolution (padding 1, stride 1 or 2)              : r3g_im2col3x3 -> [N*Ho*Wo, 9*C] rows -> r3g_linear,
 // and the align_corners=True bilinear resampling between the fusion stages (custom_interpolate, dpt_head.py:459-484) is

@@ -22,7 +22,6 @@ extern "C" int r3g_create(int device, r3g_ctx** out) {
     return R3G_E_CUDA;
   }
   *out = ctx;
-  ctx->gemm_2cta = -1;
   ctx->pdl = -1;
   // the caller's current device is left as it was (the entry points switch to ctx->device for their own duration)
   struct Restore {
@@ -34,8 +33,8 @@ extern "C" int r3g_create(int device, r3g_ctx** out) {
   cudaDeviceProp prop;
   R3G_CUDA_OK(ctx, cudaGetDeviceProperties(&prop, device));
   ctx->num_sms = prop.multiProcessorCount;
-  if (prop.major != 10) {
-    return r3g_fail(ctx, R3G_E_CUDA, "r3g_create: device %d is sm_%d%d; this library is sm_100a only", device,
+  if (prop.major != 9 || prop.minor != 0) {
+    return r3g_fail(ctx, R3G_E_CUDA, "r3g_create: device %d is sm_%d%d; this library is sm_90a only", device,
                     prop.major, prop.minor);
   }
   void* fn = nullptr;

@@ -1,20 +1,17 @@
-// r3g_linear: Y = epilogue(X . W^T + bias) on the 5th-gen tensor cores.
+// r3g_linear: Y = epilogue(X . W^T + bias) on the Hopper tensor cores (wgmma).
 //
-// Persistent, warp-specialised sm_100a kernel:
-//   warp 0      TMA producer   (cp.async.bulk.tensor, 128B-swizzled K-major tiles of X and W into a smem ring)
-//   warp 1      MMA issuer     (one elected thread: tcgen05.mma cta_group::1 kind::f16, M=128, N=BN, K=16;
-//                               fp32 accumulators in TMEM, double-buffered so the epilogue of tile i overlaps
-//                               the main loop of tile i+1)
-//   warps 2..5  epilogue       (tcgen05.ld 32x32b: one accumulator row per thread; bias, GELU, gate*y+residual,
-//                               fp16/fp32 conversion, 16-byte global stores)
+// Warp-specialised sm_90a kernel, one 128 x BN output tile per CTA:
+//   warp 8      TMA producer   (cp.async.bulk.tensor, 128B-swizzled K-major tiles of X and W into a smem ring)
+//   warps 0..7  two consumer warpgroups (wgmma.mma_async m64nBNk16, fp16 in, fp32 accumulators in registers; warpgroup
+//               g computes rows [64 g, 64 g + 64) of the tile).  After the main loop the accumulators are staged as an
+//               fp32 tile in the (then idle) operand ring and each of the 256 threads runs the epilogue for one row and
+//               half of the columns: bias, GELU, gate*y+residual, fp16/fp32 conversion, 16-byte global stores.
 // Covers every nn.Linear on the hot path: DiT qkv/proj/mlp/linear1/linear2 (hunyuan3ddit.py:196-216,259-267),
 // ShapeVAE c_qkv/c_proj/c_fc (attention_blocks.py:166-182,345-363), geo-decoder query_proj/c_q/c_kv/c_proj/mlp
 // (attention_blocks.py:250-261,484-494).
 #include <cuda_fp16.h>
-#include <stdlib.h>
 #include <string.h>
 
-#include <cstdio>
 #include "r3g_internal.h"
 #include "r3g_ptx.cuh"
 
@@ -24,8 +21,8 @@ using namespace r3g;
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 halfs = one 128-byte swizzle row
-constexpr int kNumEpilogueWarps = 8;   // two per TMEM lane quadrant, each owning half of the tile's columns
-constexpr int kNumThreads = 64 + 32 * kNumEpilogueWarps;
+constexpr int kNumEpilogueWarps = 8;   // the two consumer warpgroups; two warps per 32-row group, one per column half
+constexpr int kNumThreads = 32 * kNumEpilogueWarps + 32;
 
 struct LinearParams {
   int M, N, K;
@@ -48,17 +45,6 @@ struct LinearParams {
   int qkn_mode, qkn_q_col0, qkn_k_col0, qkn_cols;
   float qkn_eps;
   const __half *qkn_q_w, *qkn_q_b, *qkn_k_w, *qkn_k_b;
-};
-
-template <int BN>
-struct Cfg {
-  static constexpr int kStageBytesA = BM * BK * 2;
-  static constexpr int kStageBytesB = BN * BK * 2;
-  static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
-  static constexpr int kStages = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int kTmemCols = (2 * BN < 32) ? 32 : 2 * BN;  // two accumulator buffers
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ +
-                                    kNumEpilogueWarps * 768 /*epilogue operand slices*/;
 };
 
 __device__ __forceinline__ float ex2f(float x) {
@@ -94,12 +80,26 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
   return 0.5f * x + 0.5f * fabsf(x) * erf_abs;   // x>0: 0.5x(1+erf), x<0: 0.5x(1-erf|.|)
 }
 
-// Epilogue operands.  The epilogue warps (two per scheduler) cannot hide an L2 round trip per 32-column chunk: the
-// first version loaded bias / gate / residual after tcgen05.wait::ld and 48 % of the kernel's stall samples sat on
-// those loads (profiles/README.md r1f).  Now each epilogue warp stages its 128-column slice of the bias row and of
-// the (at most two) gate rows its 32 rows can belong to in its own 768 bytes of shared memory while it waits for the
-// accumulator, and the fp16 residual -- the only per-thread operand -- is fetched one chunk ahead of its use.
+// Epilogue operands.  An L2 round trip per 32-column chunk would stall the epilogue, so each epilogue warp stages its
+// (at most 128-column) slice of the bias row and of the (at most two) gate rows its 32 rows can belong to in its own
+// 768 bytes of shared memory before the main loop, and the fp16 residual -- the only per-thread operand -- is fetched
+// one chunk ahead of its use.
 constexpr int kEpiSmemPerWarp = 768;   // uint4 [0,16) bias, [16,32) gate row of lane 0's batch, [32,48) of lane 31's
+template <int BN>
+struct Cfg {
+  static constexpr int kStageBytesA = BM * BK * 2;
+  static constexpr int kStageBytesB = BN * BK * 2;
+  static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
+  // 128-column tiles keep a 3-deep ring (96 KB) so that two CTAs share an SM and one's epilogue overlaps the other's
+  // main loop; 256-column tiles (one CTA per SM) take a 4-deep ring.
+  static constexpr int kStages = BN == 256 ? 4 : 3;
+  static constexpr int kMinBlocks = BN == 256 ? 1 : 2;
+  static constexpr int kLdStage = BN + 4;   // floats per row of the staged accumulator tile (16 B skew per row)
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ +
+                                    kNumEpilogueWarps * kEpiSmemPerWarp /*epilogue operand slices*/;
+  static_assert(BM * kLdStage * 4 <= kStages * kStageBytes, "the staged accumulator tile must fit in the ring");
+};
+
 struct ChunkOperands {
   uint4 res[4];
 };
@@ -325,184 +325,157 @@ __device__ __forceinline__ int qkn_range(const LinearParams& p, int n0) {
 }
 
 template <int BN>
-__global__ void __launch_bounds__(kNumThreads, 1)
+__device__ __forceinline__ void wgmma_tile(float* acc, uint64_t da, uint64_t db) {
+  if constexpr (BN == 256) wgmma_m64n256k16_ss(acc, da, db, 1u);
+  else wgmma_m64n128k16_ss(acc, da, db, 1u);
+}
+
+template <int BN>
+__global__ void __launch_bounds__(kNumThreads, Cfg<BN>::kMinBlocks)
 linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant__ CUtensorMap tmap_w0,
               const __grid_constant__ CUtensorMap tmap_x1, const __grid_constant__ CUtensorMap tmap_w1,
               const __grid_constant__ LinearParams p0, const __grid_constant__ LinearParams p1) {
-  // Two problems may share one persistent launch (r3g_linear_args.group_next: the img and txt streams of a
-  // DoubleStreamBlock): tiles [0, tiles0) belong to p0, the rest to p1 (p1.tiles_m == 0: no second problem).
+  // Two problems may share one launch (r3g_linear_args.group_next: the img and txt streams of a DoubleStreamBlock):
+  // tiles [0, tiles0) belong to p0, the rest to p1 (p1.tiles_m == 0: no second problem).
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atoms
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
   uint64_t* empty_bar = full_bar + C::kStages;
-  uint64_t* tmem_full_bar = empty_bar + C::kStages;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;       // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
   uint8_t* epi_smem = smem + C::kStages * C::kStageBytes + 256;   // per-epilogue-warp operand slices
+  float* acc_smem = reinterpret_cast<float*>(smem);               // the staged accumulator tile (after the main loop)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int tiles0 = p0.tiles_m * p0.tiles_n;
-  const int num_tiles = tiles0 + p1.tiles_m * p1.tiles_n;
+  const int tile = blockIdx.x;
+  const bool second = tile >= tiles0;
+  const LinearParams& p = second ? p1 : p0;
+  const int lt = second ? tile - tiles0 : tile;
+  const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
+  const int sg = tm / p.tiles_per_seg;
+  const int num_k_blocks = (p.K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_x0);
-    tma_prefetch_desc(&tmap_w0);
-    if (p1.tiles_m) {
-      tma_prefetch_desc(&tmap_x1);
-      tma_prefetch_desc(&tmap_w1);
-    }
+  if (warp == kNumEpilogueWarps && lane == 0) {
+    tma_prefetch_desc(second ? &tmap_x1 : &tmap_x0);
+    tma_prefetch_desc(second ? &tmap_w1 : &tmap_w0);
     for (int s = 0; s < C::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], kNumEpilogueWarps * 32);
+      mbar_init(&empty_bar[s], 32 * kNumEpilogueWarps);   // every consumer thread releases the slot
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::kTmemCols>(tmem_base_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
-  pdl_wait();      // everything above overlapped the previous kernel's tail; its results are visible from here on
-  pdl_trigger();   // persistent grid, one CTA per SM: the next kernel's CTAs become resident as ours retire
+  pdl_wait();   // everything above overlapped the previous kernel's tail; its results are visible from here on
 
-  if (warp == 0) {
+  if (warp == kNumEpilogueWarps) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
+      const CUtensorMap* tmap_x = second ? &tmap_x1 : &tmap_x0;
+      const CUtensorMap* tmap_w = second ? &tmap_w1 : &tmap_w0;
+      const int l0 = (tm % p.tiles_per_seg) * BM;
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const bool second = tile >= tiles0;
-        const LinearParams& p = second ? p1 : p0;
-        const CUtensorMap* tmap_x = second ? &tmap_x1 : &tmap_x0;
-        const CUtensorMap* tmap_w = second ? &tmap_w1 : &tmap_w0;
-        const int lt = second ? tile - tiles0 : tile;
-        const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
-        const int sg = tm / p.tiles_per_seg, l0 = (tm % p.tiles_per_seg) * BM;
-        const int num_k_blocks = (p.K + BK - 1) / BK;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * C::kStageBytes;
-          uint8_t* sb = sa + C::kStageBytesA;
-          mbar_expect_tx(&full_bar[stage], C::kStageBytes);
-          tma_load_3d(sa, tmap_x, &full_bar[stage], kb * BK, l0, sg, kEvictFirst);
-          tma_load_2d(sb, tmap_w, &full_bar[stage], kb * BK, tn * BN, kEvictLast);
-          if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_f16(BM, BN, false, false);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int num_k_blocks = ((tile >= tiles0 ? p1.K : p0.K) + BK - 1) / BK;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
       for (int kb = 0; kb < num_k_blocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = smem_u32(smem + stage * C::kStageBytes);
-          const uint32_t sb = sa + C::kStageBytesA;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = umma_desc_sw128(sa + k * 32, 1024, 16);
-            const uint64_t db = umma_desc_sw128(sb + k * 32, 1024, 16);
-            umma_ss(d_tmem, da, db, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);                       // frees the smem slot when the MMAs retire
-          if (kb == num_k_blocks - 1) umma_commit(&tmem_full_bar[acc]);  // accumulator complete
-        }
-        __syncwarp();
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * C::kStageBytes;
+        uint8_t* sb = sa + C::kStageBytesA;
+        mbar_expect_tx(&full_bar[stage], C::kStageBytes);
+        tma_load_3d(sa, tmap_x, &full_bar[stage], kb * BK, l0, sg, kEvictFirst);
+        tma_load_2d(sb, tmap_w, &full_bar[stage], kb * BK, tn * BN, kEvictLast);
         if (++stage == C::kStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9)
-    const int quad = warp & 3;               // TMEM lane quadrant this warp may read
-    const int col_half = (warp - 2) >> 2;    // which half of the tile's columns this warp owns
-    const int row_in_tile = quad * 32 + lane;
-    uint4* wsm = reinterpret_cast<uint4*>(epi_smem + (warp - 2) * kEpiSmemPerWarp);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const bool second = tile >= tiles0;
-      const LinearParams& p = second ? p1 : p0;
-      const int lt = second ? tile - tiles0 : tile;
-      const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int sg = tm / p.tiles_per_seg;
-      const int l = (tm % p.tiles_per_seg) * BM + row_in_tile;  // row inside the segment
-      const bool row_ok = l < p.seg_len;
-      const int r = sg * p.seg_len + l;                          // logical row
-      const int64_t out_row = (int64_t)sg * p.y_seg_stride + l;
-      const __half* gate_row = p.gate ? p.gate + (int64_t)(row_ok ? r / p.gate_rows : 0) * p.gate_ld : nullptr;
-      // stage the warp's bias / gate slices while the accumulator is still being produced
-      const int l0 = l - lane, l31 = min(l0 + 31, p.seg_len - 1);
-      const int ncol0 = tn * BN + col_half * (BN / 2);
-      int gsel = -1;
-      if (l0 < p.seg_len)
-        gsel = stage_tile_operands(p, wsm, lane, ncol0, BN / 2, sg * p.seg_len + l0, sg * p.seg_len + l31,
-                                   row_ok ? r : sg * p.seg_len + l31);
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      ChunkOperands pre;
-      bool have_pre = false;
-#pragma unroll 1
-      for (int c0 = col_half * (BN / 2); c0 < (col_half + 1) * (BN / 2); c0 += 32) {
-        const int n0 = tn * BN + c0;
-        if (n0 >= p.N) break;  // warp-uniform
-        const uint4* sbias = wsm + ((c0 - col_half * (BN / 2)) >> 3);
-        uint32_t v[32];
-        tmem_ld32(tmem_addr(tmem_base, quad * 32, acc * BN + c0), v);
-        const int nr = (BN >= 128 && (c0 & 32) == 0) ? qkn_range(p, n0) : -1;   // warp-uniform
-        if (nr >= 0) {
-          uint32_t v1[32];
-          tmem_ld32(tmem_addr(tmem_base, quad * 32, acc * BN + c0 + 32), v1);
-          tmem_ld_wait();
-          if (row_ok)
-            epilogue_qknorm(p, v, v1, out_row, n0, nr ? p.qkn_k_w : p.qkn_q_w, nr ? p.qkn_k_b : p.qkn_q_b, sbias);
-          c0 += 32;
-          have_pre = false;
-          continue;
-        }
-        if (!have_pre && row_ok) prefetch_residual(p, out_row, n0, pre);
-        const int c1 = c0 + 32;   // the next chunk of this warp's column half, if it is an ordinary one
-        const bool more = c1 < (col_half + 1) * (BN / 2) && tn * BN + c1 < p.N &&
-                          !(BN >= 128 && (c1 & 32) == 0 && qkn_range(p, tn * BN + c1) >= 0);
-        tmem_ld_wait();
-        if (row_ok)
-          epilogue_chunk(p, v, r, out_row, n0, sbias, gsel >= 0 ? sbias + 16 + 16 * gsel : nullptr, gate_row, pre,
-                         more ? tn * BN + c1 : -1);
-        have_pre = more;
-      }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty_bar[acc]);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<C::kTmemCols>(tmem_base);
+  // -------------------------------------------------------------------- consumers (warps 0..7)
+  const int wg = warp >> 2;                     // warpgroup: MMA rows [64 wg, 64 wg + 64)
+  uint4* wsm = reinterpret_cast<uint4*>(epi_smem + warp * kEpiSmemPerWarp);
+  // stage the warp's bias / gate slices before the main loop: the loads land while the tensor cores work.  The
+  // row-derived epilogue values are recomputed after the loop instead of being held in registers across it.
+  int gsel = -1;
+  {
+    const int row_in_tile = threadIdx.x & (BM - 1), col_half = threadIdx.x >> 7;
+    const int l = (tm % p.tiles_per_seg) * BM + row_in_tile;
+    const int l0 = l - lane, l31 = min(l0 + 31, p.seg_len - 1);
+    if (l0 < p.seg_len)
+      gsel = stage_tile_operands(p, wsm, lane, tn * BN + col_half * (BN / 2), BN / 2, sg * p.seg_len + l0,
+                                 sg * p.seg_len + l31, l < p.seg_len ? sg * p.seg_len + l : sg * p.seg_len + l31);
+  }
+
+  {
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * C::kStageBytes) + wg * 64 * 128;
+      const uint32_t sb = smem_u32(smem + stage * C::kStageBytes + C::kStageBytesA);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        wgmma_tile<BN>(acc, gmma_desc_sw128(sa + k * 32, 1024, 16), gmma_desc_sw128(sb + k * 32, 1024, 16));
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot goes back to the producer
+      if (kb > 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence<BN / 2>(acc);
+    named_bar_sync(1, 32 * kNumEpilogueWarps);   // both warpgroups are done reading the ring
+    const int w4 = warp & 3;
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = wg * 64 + w4 * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+      const int col = 8 * (i >> 2) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(acc_smem + row * C::kLdStage + col) = make_float2(acc[i], acc[i + 1]);
+    }
+    named_bar_sync(1, 32 * kNumEpilogueWarps);
+  }
+
+  // -------------------------------------------------------------------- epilogue: one row, half of the columns
+  const int row_in_tile = threadIdx.x & (BM - 1);   // epilogue row
+  const int col_half = threadIdx.x >> 7;        // which half of the tile's columns this thread's epilogue owns
+  const int l = (tm % p.tiles_per_seg) * BM + row_in_tile;  // row inside the segment
+  const bool row_ok = l < p.seg_len;
+  const int r = sg * p.seg_len + l;                          // logical row
+  const int64_t out_row = (int64_t)sg * p.y_seg_stride + l;
+  const __half* gate_row = p.gate ? p.gate + (int64_t)(row_ok ? r / p.gate_rows : 0) * p.gate_ld : nullptr;
+  const float* srow = acc_smem + row_in_tile * C::kLdStage;
+  ChunkOperands pre;
+  bool have_pre = false;
+#pragma unroll 1
+  for (int c0 = col_half * (BN / 2); c0 < (col_half + 1) * (BN / 2); c0 += 32) {
+    const int n0 = tn * BN + c0;
+    if (n0 >= p.N) break;  // warp-uniform
+    const uint4* sbias = wsm + ((c0 - col_half * (BN / 2)) >> 3);
+    const uint32_t* v = reinterpret_cast<const uint32_t*>(srow + c0);
+    const int nr = ((c0 & 32) == 0) ? qkn_range(p, n0) : -1;   // warp-uniform
+    if (nr >= 0) {
+      if (row_ok)
+        epilogue_qknorm(p, v, v + 32, out_row, n0, nr ? p.qkn_k_w : p.qkn_q_w, nr ? p.qkn_k_b : p.qkn_q_b, sbias);
+      c0 += 32;
+      have_pre = false;
+      continue;
+    }
+    if (!have_pre && row_ok) prefetch_residual(p, out_row, n0, pre);
+    const int c1 = c0 + 32;   // the next chunk of this thread's column half, if it is an ordinary one
+    const bool more = c1 < (col_half + 1) * (BN / 2) && tn * BN + c1 < p.N &&
+                      !((c1 & 32) == 0 && qkn_range(p, tn * BN + c1) >= 0);
+    if (row_ok)
+      epilogue_chunk(p, v, r, out_row, n0, sbias, gsel >= 0 ? sbias + 16 + 16 * gsel : nullptr, gate_row, pre,
+                     more ? tn * BN + c1 : -1);
+    have_pre = more;
   }
 }
 
-// One problem of a launch: tensor maps + kernel parameters.  tile_m = rows per tile (128, or 256 for the CTA pair),
-// box_n = rows of W one CTA fetches per k-block, bn = output columns per tile.
+// One problem of a launch: tensor maps + kernel parameters.  tile_m = rows per tile, box_n = rows of W one CTA fetches
+// per k-block, bn = output columns per tile.
 struct Problem {
   LinearParams p;
   CUtensorMap tx, tw;
@@ -558,244 +531,15 @@ int launch_linear(r3g_ctx* ctx, const r3g_linear_args* a, const r3g_linear_args*
   rc = make_problem(ctx, b, BM, BN, BN, pb);
   if (rc) return rc;
   if (!b) { pb.tx = pa.tx; pb.tw = pa.tw; }
-  constexpr unsigned kAttrBit = BN == 256 ? R3G_ATTR_LINEAR256 : BN == 128 ? R3G_ATTR_LINEAR128 : R3G_ATTR_LINEAR64;
+  constexpr unsigned kAttrBit = BN == 256 ? R3G_ATTR_LINEAR256 : R3G_ATTR_LINEAR128;
   if (!(ctx->attr_done & kAttrBit)) {
     R3G_CUDA_OK(ctx, cudaFuncSetAttribute(linear_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           C::kSmemBytes));
     ctx->attr_done |= kAttrBit;
   }
   const int tiles = pa.p.tiles_m * pa.p.tiles_n + pb.p.tiles_m * pb.p.tiles_n;
-  const int grid = tiles < ctx->num_sms ? tiles : ctx->num_sms;
-  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, linear_kernel<BN>, dim3(grid), dim3(kNumThreads), C::kSmemBytes, s, pa.tx, pa.tw,
+  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, linear_kernel<BN>, dim3(tiles), dim3(kNumThreads), C::kSmemBytes, s, pa.tx, pa.tw,
                                    pb.tx, pb.tw, pa.p, pb.p));
-  R3G_LAUNCH_OK(ctx);
-  return R3G_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// 2-CTA variant (cta_group::2): a CTA pair (cluster of 2 on one TPC) computes a 256 x 256 tile.  Each CTA stages
-// ITS 128 rows of X and ITS 128 of the 256 W rows (32 KB per k-block instead of 48 KB), the leader's single thread
-// issues tcgen05.mma.cta_group::2 (M = 256) which reads both CTAs' shared memory, and each CTA's TMEM holds its own
-// 128 accumulator rows.  One third less L2 -> SMEM traffic per FLOP than the 128 x 256 single-CTA tile, which is
-// what bounds that kernel (12 TB/s of L2 bandwidth at 1.0 PFLOP/s), and room for a 6-deep ring.
-constexpr int kStages2 = 6;
-constexpr int kStageBytes2 = BM * BK * 2 + 128 * BK * 2;       // 16 KB of X + 16 KB of W per CTA
-constexpr int kSmemBytes2 = kStages2 * kStageBytes2 + 1024 + 256 + kNumEpilogueWarps * 768;
-constexpr int BN2 = 256;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kNumThreads, 1)
-linear_kernel_2cta(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant__ CUtensorMap tmap_w0,
-                   const __grid_constant__ CUtensorMap tmap_x1, const __grid_constant__ CUtensorMap tmap_w1,
-                   const __grid_constant__ LinearParams p0, const __grid_constant__ LinearParams p1) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages2 * kStageBytes2);
-  uint64_t* empty_bar = full_bar + kStages2;
-  uint64_t* tmem_full_bar = empty_bar + kStages2;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;     // [2]  (leader's copy is the one the MMA warp waits on)
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  uint8_t* epi_smem = smem + kStages2 * kStageBytes2 + 256;   // per-epilogue-warp operand slices
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();           // rank inside the CTA pair
-  const bool leader = cta_rank == 0;
-  const int tiles0 = p0.tiles_m * p0.tiles_n;              // tiles [0, tiles0): problem 0, the rest: problem 1
-  const int num_tiles = tiles0 + p1.tiles_m * p1.tiles_n;
-  const int cluster_id = blockIdx.x / 2, num_clusters = gridDim.x / 2;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_x0);
-    tma_prefetch_desc(&tmap_w0);
-    if (p1.tiles_m) {
-      tma_prefetch_desc(&tmap_x1);
-      tma_prefetch_desc(&tmap_w1);
-    }
-    for (int s = 0; s < kStages2; ++s) {
-      mbar_init(&full_bar[s], 1);    // the leader's expect_tx arrival; both CTAs' TMA bytes complete on it
-      mbar_init(&empty_bar[s], 1);   // the leader's multicast tcgen05.commit
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], 2 * kNumEpilogueWarps);  // one arrival per epilogue warp of both CTAs
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm<512>(tmem_base_smem);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
-  pdl_wait();
-  pdl_trigger();
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs)
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        const bool second = tile >= tiles0;
-        const LinearParams& p = second ? p1 : p0;
-        const CUtensorMap* tmap_x = second ? &tmap_x1 : &tmap_x0;
-        const CUtensorMap* tmap_w = second ? &tmap_w1 : &tmap_w0;
-        const int lt = second ? tile - tiles0 : tile;
-        const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
-        const int sg = tm / p.tiles_per_seg, l0 = (tm % p.tiles_per_seg) * 256 + (int)cta_rank * BM;
-        const int num_k_blocks = (p.K + BK - 1) / BK;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * kStageBytes2;
-          uint8_t* sb = sa + BM * BK * 2;
-          // the peer only issues its loads: its bytes are accounted on the leader's barrier (a phase cannot
-          // complete before they land because the leader armed it with the bytes of BOTH CTAs)
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * kStageBytes2);
-          tma_load_3d_2sm(sa, tmap_x, &full_bar[stage], kb * BK, l0, sg, kEvictFirst);
-          tma_load_2d_2sm(sb, tmap_w, &full_bar[stage], kb * BK, tn * BN2 + (int)cta_rank * 128, kEvictLast);
-          if (++stage == kStages2) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only)
-    if (leader) {
-      constexpr uint32_t idesc = umma_idesc_f16(256, BN2, false, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-        const int num_k_blocks = ((tile >= tiles0 ? p1.K : p0.K) + BK - 1) / BK;
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN2;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (lane == 0) {
-            const uint32_t sa = smem_u32(smem + stage * kStageBytes2);
-            const uint32_t sb = sa + BM * BK * 2;
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              umma_ss_2sm(d_tmem, umma_desc_sw128(sa + k * 32, 1024, 16), umma_desc_sw128(sb + k * 32, 1024, 16), idesc,
-                          (kb | k) ? 1u : 0u);
-            umma_commit_2sm(&empty_bar[stage], 3);
-            if (kb == num_k_blocks - 1) umma_commit_2sm(&tmem_full_bar[acc], 3);
-          }
-          __syncwarp();
-          if (++stage == kStages2) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (both CTAs, own 128 rows)
-    const int quad = warp & 3;
-    const int col_half = (warp - 2) >> 2;
-    const int row_in_tile = (int)cta_rank * BM + quad * 32 + lane;
-    uint4* wsm = reinterpret_cast<uint4*>(epi_smem + (warp - 2) * kEpiSmemPerWarp);
-    int it = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-      const bool second = tile >= tiles0;
-      const LinearParams& p = second ? p1 : p0;
-      const int lt = second ? tile - tiles0 : tile;
-      const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int sg = tm / p.tiles_per_seg;
-      const int l = (tm % p.tiles_per_seg) * 256 + row_in_tile;
-      const bool row_ok = l < p.seg_len;
-      const int r = sg * p.seg_len + l;                          // logical row
-      const int64_t out_row = (int64_t)sg * p.y_seg_stride + l;
-      const __half* gate_row = p.gate ? p.gate + (int64_t)(row_ok ? r / p.gate_rows : 0) * p.gate_ld : nullptr;
-      // stage the warp's bias / gate slices while the accumulator is still being produced
-      const int l0 = l - lane, l31 = min(l0 + 31, p.seg_len - 1);
-      const int ncol0 = tn * BN2 + col_half * (BN2 / 2);
-      int gsel = -1;
-      if (l0 < p.seg_len)
-        gsel = stage_tile_operands(p, wsm, lane, ncol0, BN2 / 2, sg * p.seg_len + l0, sg * p.seg_len + l31,
-                                   row_ok ? r : sg * p.seg_len + l31);
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      ChunkOperands pre;
-      bool have_pre = false;
-#pragma unroll 1
-      for (int c0 = col_half * (BN2 / 2); c0 < (col_half + 1) * (BN2 / 2); c0 += 32) {
-        const int n0 = tn * BN2 + c0;
-        if (n0 >= p.N) break;  // warp-uniform
-        const uint4* sbias = wsm + ((c0 - col_half * (BN2 / 2)) >> 3);
-        uint32_t v[32];
-        tmem_ld32(tmem_addr(tmem_base, quad * 32, acc * BN2 + c0), v);
-        const int nr = (BN2 >= 128 && (c0 & 32) == 0) ? qkn_range(p, n0) : -1;   // warp-uniform
-        if (nr >= 0) {
-          uint32_t v1[32];
-          tmem_ld32(tmem_addr(tmem_base, quad * 32, acc * BN2 + c0 + 32), v1);
-          tmem_ld_wait();
-          if (row_ok)
-            epilogue_qknorm(p, v, v1, out_row, n0, nr ? p.qkn_k_w : p.qkn_q_w, nr ? p.qkn_k_b : p.qkn_q_b, sbias);
-          c0 += 32;
-          have_pre = false;
-          continue;
-        }
-        if (!have_pre && row_ok) prefetch_residual(p, out_row, n0, pre);
-        const int c1 = c0 + 32;   // the next chunk of this warp's column half, if it is an ordinary one
-        const bool more = c1 < (col_half + 1) * (BN2 / 2) && tn * BN2 + c1 < p.N &&
-                          !(BN2 >= 128 && (c1 & 32) == 0 && qkn_range(p, tn * BN2 + c1) >= 0);
-        tmem_ld_wait();
-        if (row_ok)
-          epilogue_chunk(p, v, r, out_row, n0, sbias, gsel >= 0 ? sbias + 16 + 16 * gsel : nullptr, gate_row, pre,
-                         more ? tn * BN2 + c1 : -1);
-        have_pre = more;
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tmem_empty_bar[acc], 0);   // the leader's MMA warp owns the wait
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
-  }
-}
-
-int launch_linear_2cta(r3g_ctx* ctx, const r3g_linear_args* a, const r3g_linear_args* b, cudaStream_t s) {
-  Problem pa, pb;
-  int rc = make_problem(ctx, a, 256, 128, BN2, pa);
-  if (rc) return rc;
-  rc = make_problem(ctx, b, 256, 128, BN2, pb);
-  if (rc) return rc;
-  if (!b) { pb.tx = pa.tx; pb.tw = pa.tw; }
-  if (!(ctx->attr_done & R3G_ATTR_LINEAR_2CTA)) {
-    R3G_CUDA_OK(ctx, cudaFuncSetAttribute(linear_kernel_2cta, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes2));
-    ctx->attr_done |= R3G_ATTR_LINEAR_2CTA;
-  }
-  // persistent grids are sized to the clusters that can be CO-RESIDENT (a GPC whose SM count is not a multiple of
-  // the cluster size leaves SMs out; a cluster that has to wait for a slot would run as a second wave)
-  if (!ctx->max_clusters2) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(ctx->num_sms / 2 * 2));
-    cfg.blockDim = dim3(kNumThreads);
-    cfg.dynamicSmemBytes = kSmemBytes2;
-    cudaLaunchAttribute at;
-    at.id = cudaLaunchAttributeClusterDimension;
-    at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-    cfg.attrs = &at;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, linear_kernel_2cta, &cfg) != cudaSuccess || n <= 0) {
-      (void)cudaGetLastError();
-      n = ctx->num_sms / 2;
-    }
-    ctx->max_clusters2 = n < ctx->num_sms / 2 ? n : ctx->num_sms / 2;
-    if (getenv("R3G_DEBUG_GEMM")) fprintf(stderr, "[r3g gemm] co-resident CTA pairs: %d\n", ctx->max_clusters2);
-  }
-  const int tiles = pa.p.tiles_m * pa.p.tiles_n + pb.p.tiles_m * pb.p.tiles_n;
-  const int clusters = tiles < ctx->max_clusters2 ? tiles : ctx->max_clusters2;
-  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, linear_kernel_2cta, dim3(2 * clusters), dim3(kNumThreads), kSmemBytes2, s, pa.tx,
-                                   pa.tw, pb.tx, pb.tw, pa.p, pb.p));
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;
 }
@@ -842,35 +586,23 @@ extern "C" int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream) 
   if (rc) return rc;
   if (b && (rc = validate_linear(ctx, b))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  // Tile choice: wave efficiency (tiles / (waves * units)) times a per-tile throughput factor measured on B200
-  // (CTA-pair 256x256: 1.08 for K <= 2048 else 0.93, 128x256: 1.0, 128x128: 0.7), over the tiles of BOTH problems of a
-  // grouped launch.  N = 1024 GEMMs with ~6k rows, for example, fill only 1.3 waves of 128x256 tiles; the img and txt
-  // streams of a DoubleStreamBlock together (6144 + 2740 rows) fill 1.95 of 2.
+  // Tile choice: wave efficiency (tiles / (waves * resident CTAs)) over the tiles of BOTH problems of a grouped launch.
+  // A 128 x 256 tile reads half the operand bytes per FLOP of a 128 x 128 one but runs one CTA per SM instead of
+  // two; it is taken unless it leaves more of the last wave idle.
   const int sms = ctx->num_sms;
-  auto eff = [&](int64_t tiles, int units, double factor) {
+  auto eff = [&](int64_t tiles, int units) {
     if (tiles <= 0) return 0.0;
     const int64_t waves = (tiles + units - 1) / units;
-    return factor * (double)tiles / (double)(waves * units);
+    return (double)tiles / (double)(waves * units);
   };
-  if (ctx->gemm_2cta < 0) {   // R3G_GEMM_2CTA=0 disables the CTA-pair kernel
-    const char* e = getenv("R3G_GEMM_2CTA");
-    ctx->gemm_2cta = (e && e[0] == '0') ? 0 : 1;
-  }
   auto tiles_of = [&](const r3g_linear_args* q, int tm, int tn) -> int64_t {
     if (!q) return 0;
     const int seg = q->seg_len > 0 ? q->seg_len : q->M;
     return (int64_t)(q->M / seg) * ((seg + tm - 1) / tm) * ((q->N + tn - 1) / tn);
   };
   const int n_min = b ? (a->N < b->N ? a->N : b->N) : a->N;
-  const int k_max = b ? (a->K > b->K ? a->K : b->K) : a->K;
-  const bool n256 = a->N % 256 == 0 && (!b || b->N % 256 == 0);
-  // measured: the CTA-pair tile wins for short K (epilogue-heavy), the single-CTA tile for K >= 4096
-  const double e2 = (ctx->gemm_2cta && n256) ? eff(tiles_of(a, 256, 256) + tiles_of(b, 256, 256), sms / 2,
-                                                    k_max <= 2048 ? 1.08 : 0.93) : 0.0;
-  const double e256 = n_min >= 256 ? eff(tiles_of(a, 128, 256) + tiles_of(b, 128, 256), sms, 1.0) : 0.0;
-  const double e128 = n_min >= 128 ? eff(tiles_of(a, 128, 128) + tiles_of(b, 128, 128), sms, 0.7) : 0.0;
-  if (e2 > 0.0 && e2 >= e256 && e2 >= e128) return launch_linear_2cta(ctx, a, b, s);
+  const double e256 = n_min >= 256 ? eff(tiles_of(a, BM, 256) + tiles_of(b, BM, 256), sms) : 0.0;
+  const double e128 = eff(tiles_of(a, BM, 128) + tiles_of(b, BM, 128), 2 * sms);
   if (e256 > 0.0 && e256 >= e128) return launch_linear<256>(ctx, a, b, s);
-  if (n_min >= 128) return launch_linear<128>(ctx, a, b, s);
-  return launch_linear<64>(ctx, a, b, s);
+  return launch_linear<128>(ctx, a, b, s);
 }

@@ -23,12 +23,10 @@ struct r3g_ctx {
   int64_t* pinned;
   // per-device lazy state (function attributes and occupancy queries are per device, a context is per device)
   unsigned attr_done;          // R3G_ATTR_* bits: cudaFuncSetAttribute already applied on this context's device
-  int max_clusters2;           // co-resident CTA pairs of linear_kernel_2cta (0 = not queried yet)
-  int gemm_2cta;               // -1 = environment not read yet; R3G_GEMM_2CTA=0 disables the CTA-pair kernel
   int pdl;                     // -1 = environment not read yet; R3G_PDL=0 disables programmatic dependent launch
 };
-enum { R3G_ATTR_ATTENTION = 1, R3G_ATTR_LINEAR64 = 2, R3G_ATTR_LINEAR128 = 4, R3G_ATTR_LINEAR256 = 8,
-       R3G_ATTR_LINEAR_2CTA = 16, R3G_ATTR_MISC0 = 32, R3G_ATTR_MISC1 = 64, R3G_ATTR_MISC2 = 128 };
+enum { R3G_ATTR_ATTENTION = 1, R3G_ATTR_LINEAR128 = 4, R3G_ATTR_LINEAR256 = 8,
+       R3G_ATTR_MISC0 = 32, R3G_ATTR_MISC1 = 64, R3G_ATTR_MISC2 = 128 };
 
 // Every ABI entry point runs with the context's device current (a kernel cannot be launched into a stream of
 // another device) and restores the caller's device on return.

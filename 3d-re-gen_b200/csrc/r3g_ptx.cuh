@@ -1,5 +1,5 @@
-// Inline-PTX wrappers for the sm_100a primitives the kernels use: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st / fences), elect, cache hints.  No CUTLASS/CuTe dependency.
+// Inline-PTX wrappers for the sm_90a primitives the kernels use: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (warpgroup MMA, descriptors, fences), elect, cache hints.  No CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -28,7 +28,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 // Programmatic dependent launch (griddepcontrol): a kernel launched with the programmatic-stream-serialization
 // attribute may start while its predecessor in the stream is still running; pdl_wait() blocks until every
-// prerequisite grid has COMPLETED and its memory is visible, so everything before it (barrier init, TMEM allocation,
+// prerequisite grid has COMPLETED and its memory is visible, so everything before it (barrier init,
 // tensor-map prefetch, staging of constant weights) overlaps the predecessor's tail.  pdl_trigger() lets the next
 // kernel in the stream begin its own prologue.  Both are no-ops for a kernel launched without the attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -45,7 +45,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
 // suspend-time hint: without it try_wait returns after a few cycles and a waiting warp spins through the issue
-// port (the attention kernel's TMA warp executed 20 % of all warp instructions that way, profiles/README.md r1f)
+// port, taking issue slots from the warps that do the work
 constexpr uint32_t kMbarSuspendHint = 0x989680u;
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -67,8 +67,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
+
+// named barrier over the first `count` threads of the CTA (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory");
+}
 
 // ----------------------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -104,155 +107,59 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ----------------------------------------------------------------------------- tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "TMEM cols");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+// ----------------------------------------------------------------------------- wgmma (warpgroup MMA)
+// A warpgroup (4 consecutive warps) issues each wgmma together.  Accumulator layout of a 64 x N fp32 tile: thread t
+// of the warpgroup holds element i (0 <= i < N/2) at row 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2),
+// column 8 (i / 4) + 2 (t % 4) + i % 2.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void wgmma_reg_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues for the CTA.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16, smem] * B[128 x 16, smem]^T, both K-major; fp16 in, fp32 accumulators in registers.
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
+// D[64 x 256] (+)= A[64 x 16, smem] * B[256 x 16, smem]^T, both K-major; fp16 in, fp32 accumulators in registers.
+__device__ __forceinline__ void wgmma_m64n256k16_ss(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 columns of 32-bit: thread t of the warp receives lane (base_lane + t), columns col..col+31.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
-
-// TMEM address: bits [31:16] lane, [15:0] column.
-__device__ __forceinline__ uint32_t tmem_addr(uint32_t base, uint32_t lane, uint32_t col) {
-  return base + (lane << 16) + col;
-}
-
-// ----------------------------------------------------------------------------- 2-CTA (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// shared::cluster addresses carry the CTA rank in bit 24: clearing it names the same offset in the pair's leader
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-// TMA load whose completion is signalled on the LEADER CTA's mbarrier (both CTAs of the pair feed one barrier).
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2, uint64_t hint = kEvictNormal) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                uint64_t hint = kEvictNormal) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-// The same, multicast: the box lands at the same smem offset of every CTA in `mask` and each destination's bytes are
-// signalled on the mbarrier of ITS pair leader (the peer-bit trick applies per destination CTA).
-__device__ __forceinline__ void tma_load_2d_2sm_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                   uint16_t mask, uint64_t hint = kEvictNormal) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      ".L2::cache_hint [%0], [%1, {%4, %5}], [%2], %3, %6;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "h"(mask), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-// arrive (count 1) on the mbarrier at the same smem offset in CTA `cta` of the cluster.  RELAXED: the callers order
-// their TMEM accesses with tcgen05 fences; a .release.cluster arrive compiles to MEMBAR.ALL.GPU (microseconds).
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(raddr) : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem, 128 rows per CTA] * B[smem, N/2 rows per CTA]; issued by the leader only.
-__device__ __forceinline__ void umma_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
+// D[64 x 64] (+)= A[64 x 16, registers] * B[16 x 64, smem], B MN-major (row-major K x N tile, transposed by
+// the instruction); a[0..3] hold the fp16 A fragment in the accumulator layout of a 64 x 16 tile.
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float* d, const uint32_t* a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
 }
-// arrive on the mbarrier at this smem offset in every CTA of `mask` once the issued MMAs have completed
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t mask = 3) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------- packed fp32 (FADD2 / FMUL2 / FFMA2)
-// Blackwell's packed fp32 pipe: two IEEE fp32 results per issued instruction, operands in aligned 64-bit register pairs.
+// ----------------------------------------------------------------------------- fp32 pairs
+// Two fp32 values in one 64-bit register pair; the arithmetic is two correctly rounded scalar operations (no
+// contraction), so results are bit-identical to the element-wise IEEE operations.
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -262,45 +169,34 @@ __device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  f2_unpack(a, a0, a1); f2_unpack(b, b0, b1); f2_unpack(c, c0, c1);
+  return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1); f2_unpack(b, b0, b1);
+  return f2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1); f2_unpack(b, b0, b1);
+  return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
-// ----------------------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (sm_100 "version 1"), see cute/arch/mma_sm100_desc.hpp for the bit layout:
-//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [49,52) base offset | [61,64) layout
-// K-major, SWIZZLE_128B: rows are 128 B (64 halfs), 8-row groups are 1024 B apart (SBO), LBO unused (1).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
+// ----------------------------------------------------------------------------- wgmma descriptors
+// Shared-memory matrix descriptor (sm_90):
+//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset | [62,64) layout (1 = SWIZZLE_128B)
+// K-major SWIZZLE_128B: rows are 128 B (64 halfs), 8-row groups are SBO = 1024 B apart, LBO unused; a 16-column K step
+// inside the 64-column swizzle atom advances the start address by 32 B.  MN-major SWIZZLE_128B (the V tile of the
+// attention kernel): 64 MN elements per 128 B row, SBO = distance between 8-row groups along K.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
-}
-
-// Instruction descriptor for kind::f16 (see UMMA::InstrDescriptor): fp16 (or bf16) inputs, fp32 accumulate.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, bool a_mn_major, bool b_mn_major,
-                                                      bool bf16 = false) {
-  return (1u << 4)                              // c_format = F32
-         | ((bf16 ? 1u : 0u) << 7)              // a_format
-         | ((bf16 ? 1u : 0u) << 10)             // b_format
-         | ((a_mn_major ? 1u : 0u) << 15)       // a_major
-         | ((b_mn_major ? 1u : 0u) << 16)       // b_major
-         | ((uint32_t)(N >> 3) << 17)           // n_dim
-         | ((uint32_t)(M >> 4) << 24);          // m_dim
 }
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {

@@ -51,10 +51,9 @@ constexpr int kLnMaxChunks = 8;  // 8 chunks * 32 lanes * 8 halfs = 2048
 
 // Rows are walked by persistent warps; the NEXT row's 16-byte loads are issued (into packed registers) before the
 // current row is reduced, so every warp always has a full row in flight.  NCH = chunks of 8 halfs per lane
-// (4: width <= 1024, 8: width <= 2048).  The arithmetic runs on Blackwell's packed fp32 pipe (FADD2 / FMUL2 / FFMA2,
-// two IEEE fp32 results per instruction) and the affine weights sit in shared memory as fp32: at 6.5 TB/s an fp16
-// LayerNorm has a budget of ~10 issue slots per element, the scalar version spent 11 and ran at 2.6 TB/s
-// (profiles/README.md r1f).
+// (4: width <= 1024, 8: width <= 2048).  The arithmetic works on fp32 pairs (f2_*, r3g_ptx.cuh) and the affine
+// weights sit in shared memory as fp32, which keeps the per-element instruction count low enough for an HBM-bound
+// fp16 LayerNorm.
 __device__ __forceinline__ uint32_t f2_to_h2(uint64_t v) {   // round a pair to packed fp16 (lo in the low half)
   float lo, hi;
   f2_unpack(v, lo, hi);
@@ -410,8 +409,8 @@ __global__ void __launch_bounds__(256) patchify_kernel(const float* __restrict__
 // ------------------------------------------------------------------------------------------- GEMV (M <= 8)
 constexpr int kGemvMaxB = 8;
 constexpr int kGemvRows = 4;   // output rows per warp, their weight loads issued together (bytes in flight)
-// The activated input vectors are staged once per block in shared memory (the first version re-evaluated
-// silu() -- an expf and a divide -- for every output row and ran at 1.0 TB/s, MUFU-bound; profiles/README.md r1f).
+// The activated input vectors are staged once per block in shared memory, so silu() -- an expf and a divide -- is
+// evaluated once per input element instead of once per output row.
 template <int BT>
 __global__ void __launch_bounds__(256) gemv_kernel(const __half* __restrict__ w, const __half* __restrict__ bias,
                                                    const __half* __restrict__ vec, int64_t vec_ld,

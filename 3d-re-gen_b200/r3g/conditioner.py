@@ -3,7 +3,7 @@ SingleImageEncoder(main_image_encoder=DinoImageEncoder) -> {'main': [B, 1370, 15
 embedding is zeros.  The reference runs transformers' Dinov2Model (40 layers, 1536 wide, 24 heads of 64, SwiGLU MLP,
 LayerScale) once per object, ~3 TFLOP.  Here `self.model` is still that HF module -- it owns the state dict a
 checkpoint loads into (pipelines.py:179-180 loads it strictly) -- but on a CUDA device the forward runs on the r3g
-kernels (SURVEY.md section 8f row 4): patchify + tcgen05 GEMM for the 14x14 patch embedding, LayerNorm, one q|k|v
+kernels (SURVEY.md section 8f row 4): patchify + wgmma GEMM for the 14x14 patch embedding, LayerNorm, one q|k|v
 projection, flash attention, projection with the LayerScale-gated residual fused in the epilogue, SwiGLU gate.
 `backend="hf"` keeps the library forward (CPU, and the parity test's other side)."""
 import torch

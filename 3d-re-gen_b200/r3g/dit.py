@@ -10,7 +10,7 @@ Data layout in HBM (per forward, B = 2 for classifier-free guidance):
                                  [q | mlp | k | v], so that after attention has written its output over q the first
                                  5*hidden columns ARE cat(attn, gelu(mlp)) -- linear2's input (:264-266), no cat
   mods  [B, sum(mod widths)]     every block's Modulation.lin output from ONE gemv per forward
-All GEMMs / attention run on tcgen05 (gemm.cu, attn.cu); LayerNorm+modulation, q/k RMS-norm are row kernels.
+All GEMMs / attention run on wgmma (gemm.cu, attn.cu); LayerNorm+modulation, q/k RMS-norm are row kernels.
 """
 
 import torch

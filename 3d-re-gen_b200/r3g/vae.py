@@ -248,6 +248,7 @@ class FlashVDMVolumeDecoding:
         if topk_mode != "mean":
             raise NotImplementedError("topk_mode='merge' (FlashVDMTopMCrossAttentionProcessor) is not mirrored")
         self.stats = {}
+        self.max_group_queries = 1 << 20   # refinement rows per decode call (workspace ~15 GB at width 1024)
 
     @staticmethod
     def _topk(n_keys):
@@ -291,7 +292,7 @@ class FlashVDMVolumeDecoding:
         v_hld = v_all[0].permute(1, 0, 2)
         n_keys = k_hld.shape[1]
         topk = self._topk(n_keys)
-        self.stats = dict(resolutions=list(resolutions), queries=[])
+        self.stats = dict(resolutions=list(resolutions), queries=[], groups=[])
 
         # ---- level 0: dense grid, processed as mini_grid_num^3 mini-grids (each one batch element of the attention)
         n0 = resolutions[0] + 1
@@ -344,19 +345,30 @@ class FlashVDMVolumeDecoding:
             starts = torch.cumsum(counts, 0) - counts
             spans = list(zip(starts.tolist(), counts.tolist()))
             n = pts.shape[0]
-            ws = geo._workspace(max(n, 1))
-            ops.points_fourier_f32(pts, ws["emb"][:n], geo.num_freqs, geo.include_pi)
+            # whole buckets are decoded in groups of at most max_group_queries rows through one workspace: the last
+            # level of octree_resolution 256 selects ~8 M points, whose all-at-once workspace would not fit in HBM
+            groups, g0, cur = [], 0, []
+            for s0, c in spans:
+                if cur and s0 + c - g0 > self.max_group_queries:
+                    groups.append((g0, s0, cur))
+                    g0, cur = s0, []
+                cur.append((s0 - g0, c))
+            groups.append((g0, n, cur))
+            self.stats["groups"].append(len(groups))
+            ws = geo._workspace(max(max(r1 - r0 for r0, r1, _ in groups), 1))
             vals = torch.empty(n, device=dev, dtype=torch.float32)
 
-            def attn_buckets(q4):
-                for s0, c in spans:
+            def attn_buckets(q4, gspans):
+                for s0, c in gspans:
                     qc = q4[:, s0:s0 + c]                          # [1, c, H, 64]
                     idx = self._select(qc.permute(0, 2, 1, 3), k_hld, topk, 50)[0]      # [H, topk]
                     gi = idx[..., None].expand(-1, -1, 64)
                     k0 = torch.gather(k_hld, 1, gi)                # [H, topk, 64]
                     v0 = torch.gather(v_hld, 1, gi)
                     ops.attention(qc, k0.permute(1, 0, 2)[None], v0.permute(1, 0, 2)[None], out=qc)
-            geo._decode(ws, n, None, vals, attention=attn_buckets)
+            for r0, r1, gspans in groups:
+                ops.points_fourier_f32(pts[r0:r1], ws["emb"][:r1 - r0], geo.num_freqs, geo.include_pi)
+                geo._decode(ws, r1 - r0, None, vals[r0:r1], attention=lambda q4, gs=gspans: attn_buckets(q4, gs))
             level = torch.full((n1, n1, n1), -10000.0, device=dev, dtype=torch.float16)
             out = torch.empty(n, device=dev, dtype=torch.float16)
             out[perm] = vals.to(torch.float16)

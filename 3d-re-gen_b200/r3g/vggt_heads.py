@@ -255,7 +255,7 @@ class DPTHead:
 
 
 class DPTHeadR3G:
-    """The DPT depth head with every convolution as a tcgen05 GEMM over channels-last fp16 feature maps (conv.cu):
+    """The DPT depth head with every convolution as a wgmma GEMM over channels-last fp16 feature maps (conv.cu):
     1x1 convolutions and the kernel == stride transposed convolutions are `ops.linear` on the pixel rows, 3x3
     convolutions `ops.im2col3x3` + `ops.linear` (ReLU / bias / residual in the GEMM epilogue), the align_corners=True
     resampling `ops.bilinear_nhwc`; the token LayerNorm is `ops.layernorm_f32in`.  The reference runs this head in float32

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the metric of BASELINE.json on B200.
+"""bench.py -- the metric of BASELINE.json on H100.
 
 Workloads (`config.workload` names the BASELINE.json config each one is):
   default / --workload shapegen   configs[1] (and [2], [4] through the flags below): one "step" = one synthetic
@@ -11,6 +11,7 @@ Workloads (`config.workload` names the BASELINE.json config each one is):
 
   python bench.py --gpus N --steps K --warmup W            # our arm (one rank per GPU under torchrun for N > 1)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on the host cores
+  python bench.py ... --dump-outputs DIR                    # also write what the last timed step returned, DIR/*.npy
 
 `value`  : objects/s with the preprocessed crop already resident in HBM and the mesh left on the device.
 `e2e`    : objects/s through the public call `pipe(image=<PIL RGBA>, ..., output_type="mesh")` with host buffers: the
@@ -65,6 +66,9 @@ def parse():
     ap.add_argument("--crops", default="synthetic", choices=["synthetic", "2400"],
                     help="2400: the 8 fixed-box crops of the reference's input_images/2400.jpg (BASELINE configs[2])")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the timed path returned in its last step (rank 0) as "
+                         "DIR/<name>.npy (float32 / float64, at most 64 MB in all: larger arrays are a seeded row sample)")
     ap.add_argument("--profile-mode", action="store_true",
                     help="warm-up + device-resident loop only (for ncu launch lists); prints no bench line")
     return ap.parse_args()
@@ -76,7 +80,30 @@ def peaks():
         d = json.load(open(path))
         return dict(tflops=d.get("bf16_tflops_sustained", d.get("bf16_tflops")), hbm=d.get("hbm_gbs"),
                     source="MEASURED_PEAKS.json (sustained cuBLAS bf16; copy bandwidth)")
-    return dict(tflops=1400.0, hbm=6650.0, source="fallback of B200_PROFILING.md")
+    return dict(tflops=989.0, hbm=3350.0, source="NVIDIA H100 SXM data sheet (dense fp16 tensor, HBM3; 700 W card)")
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: array} as out_dir/<name>.npy in float32 (float64 stays float64, integers become float64, which holds
+    them exactly).  An array above its share of DUMP_LIMIT_BYTES is flattened to rows of its last axis and replaced by
+    a fixed, seeded sample of those rows (sorted, so row order is kept); <name>_rows.npy records which rows were kept."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v) for k, v in arrays.items()}
+    arrays = {k: v.astype(np.float64 if v.dtype in (np.float64, np.int64, np.int32) else np.float32)
+              for k, v in arrays.items()}
+    share = DUMP_LIMIT_BYTES // (2 * max(len(arrays), 1))      # half the budget is headroom for the row indices
+    for name, a in arrays.items():
+        if a.nbytes > share and a.ndim >= 1 and a.size > 1:
+            a = a.reshape(-1, a.shape[-1]) if a.ndim > 1 else a
+            row_bytes = max(a.nbytes // a.shape[0], 1)
+            keep = np.sort(np.random.default_rng(0).choice(a.shape[0], size=max(share // row_bytes, 1), replace=False))
+            np.save(os.path.join(out_dir, f"{name}_rows.npy"), keep.astype(np.float64))
+            a = a[keep]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 class ClockSampler:
@@ -194,15 +221,8 @@ def reference_arm(args):
     print(json.dumps(line))
 
 
-# DRAM traffic of the DiT forward's GEMM launches: `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum` over one
-# forward (tools/prof_dit_gemm.py), averaged per launch like `achieved`; the committed capture is named beside it.
-GEMM_TRAFFIC_NCU = {"source": "profiles/r2d_ncu_dit_gemm_traffic.csv.gz (131 launches of one forward, cold L2 per launch "
-                              "under ncu: an upper bound of the in-graph traffic)",
-                    "dram_bytes_per_launch": 85.34e6}
-
-
 def instrumented_linear_roofline(pipe, cond, peak_tflops):
-    """Dominant kernel = the tcgen05 GEMM (every nn.Linear of the DiT: ~46 % of the step in the ncu launch list).
+    """Dominant kernel = the wgmma GEMM (every nn.Linear of the DiT).
     Its launches are isolated from the other kernels of the forward -- same weights, same order, same shapes and
     epilogues -- by recording one eager forward's r3g_linear calls and re-issuing exactly those into a CUDA graph,
     replayed between CUDA events on the launching stream.  achieved = sum of 2*M*N*K over the launches / elapsed."""
@@ -257,10 +277,9 @@ def instrumented_linear_roofline(pipe, cond, peak_tflops):
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / reps
     achieved = flops / ms / 1e9
-    return {"bound": "tensor", "kernel": "linear_kernel / linear_kernel_2cta (tcgen05 GEMM, gemm.cu): the DiT forward's launches",
+    return {"bound": "tensor", "kernel": "linear_kernel (wgmma GEMM, gemm.cu): the DiT forward's launches",
             "launches_timed": len(calls), "gemm_problems": len(probs), "achieved": achieved, "peak": peak_tflops, "unit": "TFLOP/s",
-            "frac": achieved / peak_tflops, "traffic": GEMM_TRAFFIC_NCU["dram_bytes_per_launch"],
-            "traffic_source": GEMM_TRAFFIC_NCU["source"], "avg_launch_ms": ms / len(calls),
+            "frac": achieved / peak_tflops, "traffic": None, "avg_launch_ms": ms / len(calls),
             "flops_per_launch_avg": flops / len(calls), "algorithmic_bytes_per_launch_avg": alg_bytes / len(calls),
             "note": "weights stream from HBM (2.2 GB per forward > L2); activations mostly L2-resident, so DRAM traffic "
                     "per launch sits below the algorithmic bytes"}
@@ -345,7 +364,7 @@ def main_shapegen(args):
     # per peer at the end of the arm (no NCCL kernel is resident while objects compute); e2e arm: per-object streaming
     # gather on a side stream into rank 0's pinned ring
     # (one GPU: each mesh streams to the pinned host ring as it finishes, under the next object's compute).  A per-object
-    # NCCL exchange during compute cost ~0.15 s per object at N = 8 (profiles/README.md r2d), so at N > 1 BOTH arms
+    # NCCL exchange during compute slows every object, so at N > 1 BOTH arms
     # keep NVLink quiet while objects compute and pay the gather -- and, for e2e, the pinned D2H of all meshes on rank 0 --
     # once, inside their timed regions.
     g_dev = MeshBatchGatherer(cap_v, cap_f, K, f"cuda:{local}") if world > 1 else None
@@ -376,6 +395,7 @@ def main_shapegen(args):
             meshes.append(m)    # object cudaMalloc fresh ~200 MB blocks (100 ms each) inside the timed region
 
     host = {"pipe_call_ms": 0.0, "gather_submit_ms": 0.0}      # host wall time of the two halves of an e2e step
+    last = {}                           # the mesh of the last timed step (--dump-outputs); no object runs after it
 
     def do_e2e(k):
         nonlocal h2d
@@ -388,6 +408,8 @@ def main_shapegen(args):
         host["pipe_call_ms"] += 1e3 * (t1 - t0) / K
         host["gather_submit_ms"] += 1e3 * (time.perf_counter() - t1) / K
         seg_e2e.append((a, mark()))
+        if k == K - 1 and args.dump_outputs:
+            last["mesh"] = m2
 
     barrier()
     if args.profile_mode:
@@ -433,6 +455,11 @@ def main_shapegen(args):
         return
     value = world * K / (ms_dev / 1000.0)
     e2e_value = world * K / (ms_e2e / 1000.0)
+    if rank == 0 and args.dump_outputs:
+        m = last.get("mesh")
+        if m is None:
+            raise SystemExit("--dump-outputs: the last timed step produced no mesh")
+        dump_outputs(args.dump_outputs, {"mesh_v": m.mesh_v.cpu().numpy(), "mesh_f": m.mesh_f.cpu().numpy()})
     if rank == 0:
         cond = pipe.encode_cond(dev_in[0], {}, True)
         roof = instrumented_linear_roofline(pipe, cond, pk["tflops"])
@@ -505,7 +532,7 @@ def main_vggt(args):
     def scene(images):
         E, Kmat, depth, conf = stage4.run_VGGT(model, images, 518)
         pts = ops.unproject(depth[..., 0].contiguous(), E, Kmat, torch.float64)
-        return pts, depth, conf
+        return pts, depth, conf, E, Kmat
 
     def barrier():
         torch.cuda.synchronize()
@@ -528,7 +555,7 @@ def main_vggt(args):
         ev[2 * k + 1].record()
         img = host_in[W + k].cuda(non_blocking=True)
         h2d += host_in[W + k].numel() * 4
-        pts, depth, conf = scene(img)
+        pts, depth, conf, extrinsic, intrinsic = scene(img)      # the cameras come back as host arrays
         host_pts.copy_(pts, non_blocking=True)
         host_dc[0].copy_(depth[..., 0], non_blocking=True)
         host_dc[1].copy_(conf, non_blocking=True)
@@ -543,6 +570,9 @@ def main_vggt(args):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_dev, ms_e2e = t.tolist()
+    if rank == 0 and args.dump_outputs:         # what the last step returned: cameras, back-projected points, depth, confidence
+        dump_outputs(args.dump_outputs, {"extrinsic": extrinsic, "intrinsic": intrinsic, "points": host_pts.numpy(),
+                                         "depth": host_dc[0].numpy(), "conf": host_dc[1].numpy()})
     if rank == 0:
         # roofline: the back-projection kernel on a shape long enough to read a bandwidth (SURVEY.md section 8d row 4:
         # the real 2 x 518^2 call is 8.6 MB = launch-latency bound)

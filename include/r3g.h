@@ -1,4 +1,4 @@
-/* r3g -- C ABI of the B200-native hot path of 3D-RE-GEN (stage 3: Hunyuan3D-2 shape generation,
+/* r3g -- C ABI of the H100-native hot path of 3D-RE-GEN (stage 3: Hunyuan3D-2 shape generation,
  * stage 4: VGGT back-projection).  The reference has no FFI of its own: its operator interface is the
  * set of Python plug points listed in SURVEY.md section 8(b).  Every entry point below names the reference
  * interface (file:line under /root/reference) it sits underneath; the Python mirror of those
@@ -74,7 +74,7 @@ int r3g_mc_classify(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, flo
 int r3g_mesh_components(r3g_ctx* ctx, const int32_t* faces, int64_t nf, int64_t nv, int32_t* labels, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Dense-contraction building blocks (tcgen05 / TMEM / TMA).  Used by the DiT, ShapeVAE and geo-decoder
+ * Dense-contraction building blocks (wgmma / TMA).  Used by the DiT, ShapeVAE and geo-decoder
  * mirrors; exported so that tests can check each against the oracle in isolation.
  *
  * r3g_linear:  Y = epilogue( X[M,K] . W[N,K]^T + bias )  -- nn.Linear semantics, fp16 in, fp32 accumulate.

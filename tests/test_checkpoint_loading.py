@@ -1,28 +1,29 @@
 """CPU: `Hunyuan3DDiTFlowMatchingPipeline.from_pretrained` on a fabricated checkpoint in the reference's layout
 ($HY3DGEN_MODELS/<repo>/<subfolder>/config.yaml + model.fp16.safetensors with `model.` / `vae.` / `conditioner.` key
-prefixes, pipelines.py:140-232).  The tensors come from modules built with the reference's own classes (small sizes), so
-the test pins the state-dict key mapping, the linear1 row permutation and the modulation packing -- the part of the
-drop-in that no GPU test can reach because no real checkpoint is reachable here."""
+prefixes, pipelines.py:140-232).  The state-dict keys and shapes are those of the reference's own classes at small sizes
+(stored by oracle/make_reference_checks.py), filled with seeded values, so the test pins the state-dict key mapping, the
+linear1 row permutation and the modulation packing -- the part of the drop-in that no GPU test can reach because no real
+checkpoint is reachable here."""
 import os
 import sys
 
-import pytest
 import torch
 import yaml
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
 def test_from_pretrained_maps_a_reference_layout_checkpoint(tmp_path, monkeypatch):
-    import ref_import
-    if not ref_import.available():
-        pytest.skip("/root/reference not present")
+    import numpy as np
     import safetensors.torch
     from transformers import Dinov2Config, Dinov2Model
-    ref_dit = ref_import.hunyuan_dit()
-    ab, _, _ = ref_import.hunyuan_autoencoders()
+    z = np.load(os.path.join(ROOT, "tests", "golden", "reference_checks.npz"))
+    g = torch.Generator().manual_seed(0)
+
+    def module_sd(name):
+        return {str(k): torch.randn(tuple(int(x) for x in shp if x > 0), generator=g) * 0.05
+                for k, shp in zip(z[f"ckpt_{name}_keys"], z[f"ckpt_{name}_shapes"])}
     H, Mh, nh = 128, 512, 2
     dit_p = dict(in_channels=64, context_in_dim=96, hidden_size=H, mlp_ratio=4.0, num_heads=nh, depth=2,
                  depth_single_blocks=3, axes_dim=[64], theta=10000, qkv_bias=True, time_factor=1000, guidance_embed=False)
@@ -31,18 +32,15 @@ def test_from_pretrained_maps_a_reference_layout_checkpoint(tmp_path, monkeypatc
     dino_p = dict(hidden_size=96, num_hidden_layers=2, num_attention_heads=2, mlp_ratio=2, patch_size=14, image_size=56,
                   use_swiglu_ffn=True, layerscale_value=1.0, qkv_bias=True, hidden_act="gelu", layer_norm_eps=1e-6)
     torch.manual_seed(0)
-    dit = ref_dit.Hunyuan3DDiT(**dit_p)
+    dit_sd = module_sd("dit")
     post_kl = torch.nn.Linear(64, 128)
-    tr = ab.Transformer(n_ctx=48, width=128, layers=2, heads=2, qkv_bias=False, qk_norm=True)
-    geo = ab.CrossAttentionDecoder(out_channels=1, num_latents=48, mlp_expand_ratio=4, downsample_ratio=1,
-                                   enable_ln_post=True, fourier_embedder=ab.FourierEmbedder(num_freqs=8, include_pi=False),
-                                   width=128, heads=2, qkv_bias=False, qk_norm=True, label_type="binary")
+    tr_sd, geo_sd = module_sd("tr"), module_sd("geo")
     dino = Dinov2Model(Dinov2Config(**dino_p))
     flat = {}
-    for k, v in dit.state_dict().items():
+    for k, v in dit_sd.items():
         flat["model." + k] = v.half().contiguous()
-    for prefix, mod in (("vae.post_kl.", post_kl), ("vae.transformer.", tr), ("vae.geo_decoder.", geo)):
-        for k, v in mod.state_dict().items():
+    for prefix, sd in (("vae.post_kl.", post_kl.state_dict()), ("vae.transformer.", tr_sd), ("vae.geo_decoder.", geo_sd)):
+        for k, v in sd.items():
             flat[prefix + k] = v.half().contiguous()
     for k, v in dino.state_dict().items():
         flat["conditioner.main_image_encoder.model." + k] = v.half().contiguous()
@@ -63,7 +61,7 @@ def test_from_pretrained_maps_a_reference_layout_checkpoint(tmp_path, monkeypatc
     monkeypatch.setenv("HY3DGEN_MODELS", str(tmp_path))
     from r3g.pipelines import Hunyuan3DDiTFlowMatchingPipeline
     pipe = Hunyuan3DDiTFlowMatchingPipeline.from_pretrained("tencent/Hunyuan3D-2", device="cpu")
-    w, sd = pipe.model.w, {k: v.half() for k, v in dit.state_dict().items()}
+    w, sd = pipe.model.w, {k: v.half() for k, v in dit_sd.items()}
     # plain tensors keep their keys
     for k in ("latent_in.weight", "cond_in.bias", "double_blocks.1.img_attn.qkv.weight", "double_blocks.0.txt_mlp.2.bias",
               "single_blocks.2.linear2.weight", "single_blocks.0.norm.key_norm.scale", "final_layer.linear.weight"):
@@ -83,10 +81,9 @@ def test_from_pretrained_maps_a_reference_layout_checkpoint(tmp_path, monkeypatc
     # VAE / geo-decoder / conditioner
     assert torch.equal(pipe.vae.w["post_kl.weight"], post_kl.weight.detach().half())
     assert torch.equal(pipe.vae.w["transformer.resblocks.1.attn.c_qkv.weight"],
-                       tr.state_dict()["resblocks.1.attn.c_qkv.weight"].half())
-    g = geo.state_dict()
-    assert torch.equal(pipe.vae.geo_decoder.w["c_kv.weight"], g["cross_attn_decoder.attn.c_kv.weight"].half())
-    assert torch.equal(pipe.vae.geo_decoder.w["query_proj.weight"][:, :51], g["query_proj.weight"].half())
+                       tr_sd["resblocks.1.attn.c_qkv.weight"].half())
+    assert torch.equal(pipe.vae.geo_decoder.w["c_kv.weight"], geo_sd["cross_attn_decoder.attn.c_kv.weight"].half())
+    assert torch.equal(pipe.vae.geo_decoder.w["query_proj.weight"][:, :51], geo_sd["query_proj.weight"].half())
     assert not pipe.vae.geo_decoder.w["query_proj.weight"][:, 51:].any()      # K padded 51 -> 64 with zeros
     enc = pipe.conditioner.main_image_encoder.model
     assert torch.equal(enc.state_dict()["encoder.layer.1.mlp.weights_in.weight"],

@@ -55,6 +55,15 @@ def test_flashvdm_two_levels_against_reference_fixture(golden_dir):
     assert dec.stats["resolutions"] == [31, 62]
     m, e, s = _report("two levels", grid.float().cpu(), ref)
     assert m >= 0.98 and e <= 3e-2 and s >= 0.995
+    # the refinement level decoded in several groups of whole buckets gives the same grid bit for bit
+    assert dec.stats["groups"] == [1]
+    split = FlashVDMVolumeDecoding("mean")
+    split.max_group_queries = max(dec.stats["queries"][1] // 5, 1)
+    grid_split = split(lat, vae.geo_decoder, bounds=1.01, num_chunks=int(z["cfg_num_chunks"]), mc_level=0.0,
+                       octree_resolution=int(z["cfg_octree"]), min_resolution=int(z["cfg_min_resolution"]),
+                       enable_pbar=False)
+    assert split.stats["groups"][0] > 1
+    assert torch.equal(grid_split.isnan(), grid.isnan()) and torch.equal(grid_split.nan_to_num(), grid.nan_to_num())
     # single dense level (every point evaluated, top-k attention per mini-grid)
     g0 = dec(lat, vae.geo_decoder, bounds=1.01, num_chunks=3000, octree_resolution=31, min_resolution=31, enable_pbar=False)
     m0, e0, s0 = _report("dense level", g0.float().cpu(), torch.from_numpy(z["grid_level0"]))

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 building blocks (r3g_linear, r3g_attention) against fp32 PyTorch on the same inputs.
+"""GPU: the wgmma building blocks (r3g_linear, r3g_attention) against fp32 PyTorch on the same inputs.
 Tolerances: fp16 inputs, fp32 accumulation, fp16 output rounding -> |err| <= 2^-10 * |y| + accumulation noise."""
 import pytest
 import torch

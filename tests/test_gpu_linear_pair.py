@@ -16,10 +16,10 @@ def _mk(M, N, K, seed, seg=None):
 
 
 @pytest.mark.parametrize("shape", [
-    dict(Ma=6144, Mb=2740, N=1024, K=1024),      # proj of a double block: CTA-pair tiles
-    dict(Ma=6144, Mb=2740, N=1024, K=4096),      # mlp.2: K = 4096 -> single-CTA 128 x 256 tiles
+    dict(Ma=6144, Mb=2740, N=1024, K=1024),      # proj of a double block: 128 x 256 tiles
+    dict(Ma=6144, Mb=2740, N=1024, K=4096),      # mlp.2: K = 4096
     dict(Ma=700, Mb=300, N=128, K=256),          # 128-wide tiles
-    dict(Ma=300, Mb=200, N=64, K=64),            # 64-wide tiles
+    dict(Ma=300, Mb=200, N=64, K=64),            # N = 64: half-filled 128-wide tiles
     dict(Ma=1000, Mb=9, N=512, K=320),           # a tiny second problem
 ])
 def test_pair_equals_two_launches(shape):

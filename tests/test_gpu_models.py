@@ -1,4 +1,4 @@
-"""GPU: the DiT / ShapeVAE / geo-decoder mirrors (fp16 storage, fp32 accumulate on tcgen05) against
+"""GPU: the DiT / ShapeVAE / geo-decoder mirrors (fp16 storage, fp32 accumulate on wgmma) against
  (a) the fixtures produced by the REFERENCE's own modules (fp32, fp16-rounded weights), and
  (b) the fp32 oracle restatement run on the same device at the reference's full widths.
 Tolerances (stated, not bit-exact -- fp16 activations): relative L2 of hidden states <= 3e-3 per block tap,

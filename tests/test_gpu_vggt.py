@@ -194,7 +194,7 @@ def test_conv_kernels_against_torch():
 
 
 def test_dpt_head_on_r3g_kernels_against_the_torch_mirror():
-    """row v6: DPTHeadR3G (every convolution a tcgen05 GEMM over NHWC fp16) vs the float32 torch mirror that
+    """row v6: DPTHeadR3G (every convolution a wgmma GEMM over NHWC fp16) vs the float32 torch mirror that
     tests/test_oracle_golden.py pins against the reference module; the real channel widths at a 70 x 84 image, and a
     small one.  Graph replay == eager."""
     from r3g.vggt_heads import DPTHead, DPTHeadR3G, random_state_dict

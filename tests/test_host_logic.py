@@ -45,22 +45,28 @@ def test_scheduler_mirror_matches_reference_fixture(golden_dir):
         sch.step(torch.zeros(1), 3, torch.zeros(1))
 
 
-def test_image_processor_against_reference_when_available():
-    import ref_import
-    if not ref_import.available():
-        pytest.skip("/root/reference not present")
-    from PIL import Image
+def _reference_checks(golden_dir):
+    return np.load(os.path.join(golden_dir, "reference_checks.npz"))
+
+
+def _sha(a):
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def test_image_processor_against_reference_when_available(golden_dir):
+    """ImageProcessorV2 (preprocessors.py) against the reference's output on the same seeded RGBA image, stored as a
+    sha256 of the image / mask tensors plus a seeded sample (oracle/make_reference_checks.py)."""
+    import make_reference_checks as mrc
     from r3g.preprocessors import ImageProcessorV2
-    ref = ref_import.hunyuan_preprocessors().ImageProcessorV2(size=512, border_ratio=0.15)
-    rng = np.random.default_rng(0)
-    rgba = np.zeros((300, 420, 4), np.uint8)
-    rgba[..., :3] = rng.integers(0, 256, (300, 420, 3))
-    yy, xx = np.mgrid[0:300, 0:420]
-    rgba[..., 3] = ((((xx - 200) / 120) ** 2 + ((yy - 160) / 90) ** 2) <= 1) * 255
-    img = Image.fromarray(rgba, "RGBA")
-    a, b = ImageProcessorV2(512, 0.15)(img), ref(img)
-    assert torch.equal(a["image"], b["image"]) and torch.equal(a["mask"], b["mask"])
-    assert a["image"].shape == (1, 3, 512, 512) and a["mask"].shape == (1, 1, 512, 512)
+    z = _reference_checks(golden_dir)
+    a = ImageProcessorV2(512, 0.15)(mrc.imgproc_input())
+    img, mask = a["image"].numpy(), a["mask"].numpy()
+    assert img.shape == (1, 3, 512, 512) and mask.shape == (1, 1, 512, 512)
+    assert tuple(z["imgproc_image_shape"]) == img.shape and tuple(z["imgproc_mask_shape"]) == mask.shape
+    assert str(img.dtype) == str(z["imgproc_image_dtype"]) and str(mask.dtype) == str(z["imgproc_mask_dtype"])
+    assert np.array_equal(img.reshape(-1)[mrc.sample_idx(img.size)], z["imgproc_image_sample"])
+    assert _sha(img) == str(z["imgproc_image_sha256"]) and _sha(mask) == str(z["imgproc_mask_sha256"])
 
 
 def test_stage3_twin_file_contract(tmp_path, monkeypatch):
@@ -97,50 +103,32 @@ def test_bench_reference_arm_contract():
     assert r1.returncode == 0 and r1.stdout.strip() == ""
 
 
-def test_conditioner_mirror_against_reference_when_available():
+def test_conditioner_mirror_against_reference_when_available(golden_dir):
     """Row a2: DinoImageEncoder (conditioner.py:57-131) -- value-range shift, Resize(bilinear, antialias) + CenterCrop +
-    Normalize, HF Dinov2Model, cls token kept; zeros as the unconditional embedding.  Same small random model in both."""
-    ref_path = "/root/reference/Hunyuan3D-2/hy3dgen/shapegen/models/conditioner.py"
-    if not os.path.exists(ref_path):
-        pytest.skip("/root/reference not present")
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("_ref_conditioner", ref_path)
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
-    sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
+    Normalize, HF Dinov2Model, cls token kept; zeros as the unconditional embedding.  The reference's small random model
+    and its outputs on seeded inputs are stored (oracle/make_reference_checks.py)."""
+    import make_reference_checks as mrc
     from r3g.conditioner import DinoImageEncoder, SingleImageEncoder
-    cfg = dict(hidden_size=32, num_hidden_layers=2, num_attention_heads=2, mlp_ratio=2, patch_size=14, image_size=56,
-               use_swiglu_ffn=True, layerscale_value=1.0, qkv_bias=True, hidden_act="gelu", layer_norm_eps=1e-6)
-    torch.manual_seed(0)
-    theirs = ref.DinoImageEncoder(config=cfg, use_cls_token=True, image_size=56)
-    mine = DinoImageEncoder(config=cfg, use_cls_token=True, image_size=56, device="cpu", dtype=torch.float32)
-    mine.model.load_state_dict(theirs.model.state_dict())
-    for shape in ((1, 3, 70, 90), (2, 3, 100, 64), (1, 3, 56, 56)):
-        img = torch.rand(shape) * 2 - 1
-        a, b = mine(img), theirs(img)
+    z = _reference_checks(golden_dir)
+    mine = DinoImageEncoder(config=mrc.COND_CFG, use_cls_token=True, image_size=56, device="cpu", dtype=torch.float32)
+    mine.model.load_state_dict({k[len("cond_w:"):]: torch.from_numpy(z[k]) for k in z.files if k.startswith("cond_w:")})
+    for i, (shape, img) in enumerate(zip(mrc.COND_SHAPES, mrc.cond_inputs())):
+        a, b = mine(img), torch.from_numpy(z[f"cond_out{i}"])
         assert a.shape == b.shape == (shape[0], 17, 32)
         assert torch.allclose(a, b, atol=1e-5, rtol=1e-5), (a - b).abs().max()
     u = SingleImageEncoder(mine).unconditional_embedding(2)["main"]
-    assert u.shape == (2, 17, 32) and not u.any() and torch.equal(u, theirs.unconditional_embedding(2))
+    assert u.shape == (2, 17, 32) and not u.any() and torch.equal(u, torch.from_numpy(z["cond_uncond"]))
 
 
-def test_near_surface_mask_against_reference_when_available():
-    """extract_near_surface_volume_fn (volume_decoders.py:29-119): the point selection of the FlashVDM levels."""
-    import ref_import
-    if not ref_import.available():
-        pytest.skip("/root/reference not present")
-    import warnings
-    _, _, vd = ref_import.hunyuan_autoencoders()
+def test_near_surface_mask_against_reference_when_available(golden_dir):
+    """extract_near_surface_volume_fn (volume_decoders.py:29-119): the point selection of the FlashVDM levels, against
+    the reference's masks on the same seeded volumes (oracle/make_reference_checks.py)."""
+    import make_reference_checks as mrc
     from r3g.vae import extract_near_surface_volume_fn
-    torch.manual_seed(0)
-    for n in (5, 9):
-        x = torch.randn(n, n, n)
-        x[torch.rand(n, n, n) < 0.25] = -10000.0
-        for alpha in (0.0, 0.3, -0.2):
-            with warnings.catch_warnings():
-                warnings.simplefilter("ignore")
-                want = vd.extract_near_surface_volume_fn(x, alpha)
-            assert torch.equal(extract_near_surface_volume_fn(x, alpha), want)
+    z = _reference_checks(golden_dir)
+    for n, x in mrc.nsm_inputs().items():
+        for j, alpha in enumerate(mrc.NSM_ALPHAS):
+            assert torch.equal(extract_near_surface_volume_fn(x.clone(), alpha), torch.from_numpy(z[f"nsm_{n}_{j}"]))
 
 
 def test_flashvdm_resolution_schedule():

@@ -1,7 +1,7 @@
 """CPU: what the built library's machine code must contain (cuobjdump on the in-tree libr3g.so).  These are the SASS
-mnemonics that prove the Blackwell paths are the ones compiled in -- tcgen05 MMAs (UTCHMMA), TMA loads (UTMALDG), TMEM
-loads/stores (LDTM/STTM), the packed fp32 pipe (FFMA2/FADD2) -- and guards against two regressions found by profiling:
-a GPU-scope membar in the GEMM pipeline (a `.release.cluster` remote arrive) and register spills in the hot kernels."""
+mnemonics that prove the Hopper paths are the ones compiled in -- warpgroup MMAs (HGMMA), TMA loads (UTMALDG), the
+register-operand P V product of the attention kernel -- and guards against two regressions: a GPU-scope membar in the
+GEMM pipeline (a `.release` arrive compiles to MEMBAR.ALL.GPU) and register spills in the hot kernels."""
 import os
 import re
 import shutil
@@ -38,40 +38,32 @@ def _one(funcs, *needles):
     return hits
 
 
-def test_gemm_is_tcgen05_tma_and_has_no_gpu_scope_membar(sass):
+def test_gemm_is_wgmma_tma_and_has_no_gpu_scope_membar(sass):
     funcs, usage = sass
-    for name in _one(funcs, "linear_kernel_2cta") + _one(funcs, "linear_kernelILi256E"):
+    for name, shape in ((_one(funcs, "linear_kernelILi128E")[0], "64x128x16"),
+                        (_one(funcs, "linear_kernelILi256E")[0], "64x256x16")):
         body = funcs[name]
-        assert "UTCHMMA" in body and "UTMALDG" in body and "LDTM" in body, name
-        # the only GPU-scope membars allowed are the two cluster barriers (start / end of the kernel)
-        ins = [ln for ln in body.split("\n") if re.match(r"\s*/\*[0-9a-f]{4}\*/", ln)]
-        for i, ln in enumerate(ins):
-            if "MEMBAR.ALL.GPU" in ln:
-                assert any("UCGABAR_ARV" in x for x in ins[i:i + 5]), \
-                    name + ": a GPU-scope membar outside the cluster barriers (a .release.cluster arrive in the pipeline?)"
-        assert sum("MEMBAR.ALL.GPU" in ln for ln in ins) <= 2, name
-        assert usage[name][1] <= 64, f"{name}: {usage[name][1]} bytes of stack (spills)"
-    assert "UTCHMMA.2CTA" in funcs[_one(funcs, "linear_kernel_2cta")[0]]
+        assert "HGMMA." + shape + ".F32" in body and "UTMALDG" in body, name
+        assert "MEMBAR.ALL.GPU" not in body, name + ": a GPU-scope membar in the pipeline"
+    name = _one(funcs, "linear_kernelILi256E")[0]
+    assert usage[name][1] == 0, f"{name}: {usage[name][1]} bytes of stack (spills)"
 
 
-def test_default_attention_uses_tmem_operand_mma_and_packed_fp32(sass):
+def test_attention_uses_register_operand_wgmma(sass):
     funcs, usage = sass
-    name = _one(funcs, "attention_kernelILb1ELb1ELi4ELi2ELb1E")[0]     # <P in TMEM, f32 exps, 1/4 poly, 2 stages, FFMA2>
+    name = _one(funcs, "attention_kernel")[0]
     body = funcs[name]
-    assert re.search(r"UTCHMMA\s+tmem\[", body), "P V must take its A operand from TMEM"
-    assert re.search(r"UTCHMMA\s+gdesc\[", body), "Q K^T is the shared-memory form"
-    for op in ("UTMALDG", "LDTM", "STTM.x32", "FFMA2", "FADD2", "MUFU.EX2", "FMNMX3"):
+    assert re.search(r"HGMMA\.64x128x16\.F32\S* R\d+, gdesc\[", body), "Q K^T is the shared-memory form"
+    assert re.search(r"HGMMA\.64x64x16\.F32\S* R\d+, R\d+, gdesc\[UR\d+\]\.tnspB", body), \
+        "P V must take its A operand from registers and V MN-major"
+    for op in ("UTMALDG", "MUFU.EX2"):
         assert op in body, op
-    assert "MUFU.EX2.F16" not in body          # the f16x2 form splits into two MUFU + a PRMT
     assert usage[name][1] == 0, "register spills in the softmax loop"
     assert "NANOSLEEP.SYNCS" in body           # mbarrier.try_wait carries the suspend-time hint
 
 
-def test_row_kernels_use_the_packed_fp32_pipe(sass):
+def test_row_kernels_move_rows_as_16_byte_accesses(sass):
     funcs, _ = sass
-    for needle in ("layernorm_kernelILi4E", "lnpost_dot_kernelILi4E"):
-        body = funcs[_one(funcs, needle)[0]]
-        assert "FFMA2" in body and "FADD2" in body, needle
     # every fp16 row moves as 16-byte accesses (a `__half2 v[4]` payload is copied member-wise: four 32-bit LDG/STG)
     for needle in ("layernorm_kernelILi4E", "lnpost_dot_kernelILi4E", "qk_norm_kernel", "gemv_kernel"):
         body = funcs[_one(funcs, needle)[0]]

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """BASELINE.json config 4: VGGT aggregator forward (S=2 frames at 518x518, the resolution the stage runs the model
-at) + point-cloud back-projection, 1 x B200.  Random weights of the VGGT-1B aggregator geometry (no checkpoint
+at) + point-cloud back-projection, 1 x H100.  Random weights of the VGGT-1B aggregator geometry (no checkpoint
 is reachable).  Prints one JSON object; the back-projection number is HBM GB/s on the [64,1022,1022] stress shape."""
 import json
 import os
@@ -11,6 +11,8 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
+sys.path.insert(0, ROOT)
+import bench  # noqa: E402
 from r3g import ops  # noqa: E402
 from r3g.vggt import Aggregator  # noqa: E402
 
@@ -74,13 +76,14 @@ def main():
     d2 = torch.rand(2, 518, 518, device="cuda") + 0.5
     ms_small = timed(lambda: ops.unproject(d2, E[:2], K[:2], torch.float64), iters=20)
     px = Sx * H * W
+    pk = bench.peaks()
     print(json.dumps({
         "config": "VGGT aggregator (DINOv2-L patch embed + 24 frame + 24 global blocks) S=2 @518^2, fp16 operands / fp32 residual",
         "aggregator_ms": ms_agg, "aggregator_algorithmic_tflop": fl / 1e12, "aggregator_tflops": fl / ms_agg / 1e9,
         "published_h100_fa3_aggregator_ms_2_frames": 50.0,
         "unproject_f64_stress_ms": ms64, "unproject_f64_GBps": px * 28 / ms64 / 1e6,
         "unproject_f32_stress_ms": ms32, "unproject_f32_GBps": px * 16 / ms32 / 1e6,
-        "unproject_2x518x518_f64_ms": ms_small, "hbm_peak_GBps": 6490.5}))
+        "unproject_2x518x518_f64_ms": ms_small, "hbm_peak_GBps": pk["hbm"], "peak_source": pk["source"]}))
 
 
 if __name__ == "__main__":

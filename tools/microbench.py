@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Kernel micro-benchmarks on one B200 (CUDA events, warm-up, L2 flush between timed launches)."""
+"""Kernel micro-benchmarks on one H100 (CUDA events, warm-up, L2 flush between timed launches)."""
 import json
 import os
 import sys
