@@ -38,12 +38,6 @@ struct AttnParams {
   float scale_log2;  // scale * log2(e)
 };
 
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 __global__ void __launch_bounds__(kThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
@@ -145,7 +139,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
       mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 2));
       const float m_new = fmaxf(m_run[rr], mx[rr] * p.scale_log2);
-      alpha[rr] = ex2(m_run[rr] - m_new);   // 0 on the first tile (m_run = -inf)
+      alpha[rr] = ex2_approx(m_run[rr] - m_new);   // 0 on the first tile (m_run = -inf)
       m_run[rr] = m_new;
       l_run[rr] *= alpha[rr];
     }
@@ -156,8 +150,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
     for (int i = 0; i < kBKV / 2; i += 2) {
       const int rr = (i >> 1) & 1;
-      const float e0 = ex2(fmaf(s[i], p.scale_log2, -m_run[rr]));
-      const float e1 = ex2(fmaf(s[i + 1], p.scale_log2, -m_run[rr]));
+      const float e0 = ex2_approx(fmaf(s[i], p.scale_log2, -m_run[rr]));
+      const float e1 = ex2_approx(fmaf(s[i + 1], p.scale_log2, -m_run[rr]));
       l_run[rr] += e0 + e1;
       pk[i >> 3][(i >> 1) & 3] = pack_half2(e0, e1);
     }
@@ -202,12 +196,10 @@ int make_qkv_map(r3g_ctx* ctx, CUtensorMap* m, const void* base, int64_t sb, int
 }  // namespace
 
 extern "C" int r3g_attention(r3g_ctx* ctx, const r3g_attention_args* a, void* stream) {
-  r3g_device_guard guard(ctx);
-  if (!ctx || !ctx->encode_tiled)
-    return r3g_fail(ctx, R3G_E_CUDA, "attention: no CUDA device (there is no CPU fallback)");
+  R3G_ENTRY(ctx, "attention");
   if (!a || !a->q || !a->k || !a->v || !a->o) return r3g_fail(ctx, R3G_E_INVALID, "attention: null argument");
   if (a->B < 1 || a->H < 1 || a->Lq < 1 || a->Lk < 1) return r3g_fail(ctx, R3G_E_INVALID, "attention: empty shape");
-  if (a->o_sl % 8 || a->o_sh % 8 || a->o_sb % 8 || ((uintptr_t)a->o) % 16)
+  if (a->o_sl % 8 || a->o_sh % 8 || a->o_sb % 8 || !r3g_aligned16(a->o))
     return r3g_fail(ctx, R3G_E_INVALID, "attention: output strides must be multiples of 8 halfs");
   CUtensorMap mq, mk, mv;
   int rc;

@@ -84,15 +84,11 @@ __global__ void __launch_bounds__(256) bilinear_nhwc_kernel(const __half* __rest
 
 }  // namespace
 
-#define R3G_CONV_GPU(ctx, name) \
-  if (!(ctx) || !(ctx)->encode_tiled) return r3g_fail((ctx), R3G_E_CUDA, name ": no CUDA device (there is no CPU fallback)"); \
-  r3g_device_guard r3g_guard_(ctx)
-
 extern "C" int r3g_im2col3x3(r3g_ctx* ctx, const void* x, void* cols, int N, int H, int W, int C, int stride, int relu_in,
                              void* stream) {
-  R3G_CONV_GPU(ctx, "im2col3x3");
-  if (!x || !cols || N < 1 || H < 1 || W < 1 || C < 8 || C % 8 || (stride != 1 && stride != 2) || (((uintptr_t)x) & 15) ||
-      (((uintptr_t)cols) & 15))
+  R3G_ENTRY(ctx, "im2col3x3");
+  if (!x || !cols || N < 1 || H < 1 || W < 1 || C < 8 || C % 8 || (stride != 1 && stride != 2) || !r3g_aligned16(x) ||
+      !r3g_aligned16(cols))
     return r3g_fail(ctx, R3G_E_INVALID, "im2col3x3: C %% 8 == 0, stride 1 or 2, 16-byte aligned buffers required");
   const int Ho = (H + 2 - 3) / stride + 1, Wo = (W + 2 - 3) / stride + 1;
   const int64_t total = (int64_t)N * Ho * Wo * 9 * (C / 8);
@@ -105,9 +101,9 @@ extern "C" int r3g_im2col3x3(r3g_ctx* ctx, const void* x, void* cols, int N, int
 
 extern "C" int r3g_bilinear_nhwc(r3g_ctx* ctx, const void* x, void* out, int N, int Hi, int Wi, int Ho, int Wo, int C,
                                  void* stream) {
-  R3G_CONV_GPU(ctx, "bilinear_nhwc");
-  if (!x || !out || N < 1 || Hi < 1 || Wi < 1 || Ho < 1 || Wo < 1 || C < 8 || C % 8 || (((uintptr_t)x) & 15) ||
-      (((uintptr_t)out) & 15))
+  R3G_ENTRY(ctx, "bilinear_nhwc");
+  if (!x || !out || N < 1 || Hi < 1 || Wi < 1 || Ho < 1 || Wo < 1 || C < 8 || C % 8 || !r3g_aligned16(x) ||
+      !r3g_aligned16(out))
     return r3g_fail(ctx, R3G_E_INVALID, "bilinear_nhwc: C %% 8 == 0 and 16-byte aligned buffers required");
   const int64_t total = (int64_t)N * Ho * Wo * (C / 8);
   const unsigned grid = (unsigned)min((total + 255) / 256, (int64_t)ctx->num_sms * 16);

@@ -59,7 +59,6 @@ extern "C" int64_t r3g_launch_count(r3g_ctx* ctx) { return ctx ? ctx->launches :
 
 int r3g_make_tmap_f16(r3g_ctx* ctx, CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                       const uint64_t* strides_bytes, const uint32_t* box) {
-  if (!ctx->encode_tiled) return r3g_fail(ctx, R3G_E_CUDA, "tensor-map encoder unavailable (no CUDA device)");
   cuuint64_t gdim[5];
   cuuint64_t gstr[5];
   cuuint32_t bx[5];
@@ -75,7 +74,7 @@ int r3g_make_tmap_f16(r3g_ctx* ctx, CUtensorMap* out, const void* base, int rank
                         (unsigned long long)strides_bytes[i]);
     }
   }
-  if (((uintptr_t)base) % 16 != 0) return r3g_fail(ctx, R3G_E_INVALID, "tensor-map base not 16-byte aligned");
+  if (!r3g_aligned16(base)) return r3g_fail(ctx, R3G_E_INVALID, "tensor-map base not 16-byte aligned");
   CUresult r = ctx->encode_tiled(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, (void*)base, gdim, gstr, bx,
                                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

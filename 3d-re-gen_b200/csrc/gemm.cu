@@ -47,11 +47,6 @@ struct LinearParams {
   const __half *qkn_q_w, *qkn_q_b, *qkn_k_w, *qkn_k_b;
 };
 
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ float rcpf(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -64,7 +59,7 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
   constexpr float b = a * 0.044715f;
   const float t = x * x;
   const float z = x * fmaf(b, t, a);          // -2u log2(e)
-  return x * rcpf(1.f + ex2f(z));
+  return x * rcpf(1.f + ex2_approx(z));
 }
 // erf-GELU: 0.5 x (1 + erf(x / sqrt 2)), erf by Abramowitz-Stegun 7.1.26 (|abs err| <= 1.5e-7).
 __device__ __forceinline__ float gelu_erf_f(float x) {
@@ -75,7 +70,7 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
   pl = fmaf(pl, t, -0.284496736f);
   pl = fmaf(pl, t, 0.254829592f);
   pl *= t;
-  const float e = ex2f(az * az * -1.4426950408889634f);
+  const float e = ex2_approx(az * az * -1.4426950408889634f);
   const float erf_abs = fmaf(-pl, e, 1.f);
   return 0.5f * x + 0.5f * fabsf(x) * erf_abs;   // x>0: 0.5x(1+erf), x<0: 0.5x(1-erf|.|)
 }
@@ -574,9 +569,8 @@ int validate_linear(r3g_ctx* ctx, const r3g_linear_args* a) {
 }  // namespace
 
 extern "C" int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream) {
-  if (!ctx || !ctx->encode_tiled) return r3g_fail(ctx, R3G_E_CUDA, "linear: no CUDA device (there is no CPU fallback)");
+  R3G_ENTRY(ctx, "linear");
   if (!a) return r3g_fail(ctx, R3G_E_INVALID, "linear: null argument");
-  r3g_device_guard guard(ctx);
   const r3g_linear_args* b = (const r3g_linear_args*)a->group_next;
   if (b && b->group_next) return r3g_fail(ctx, R3G_E_INVALID, "linear: at most two problems per launch");
   if (a->M <= 0) { a = b; b = nullptr; }

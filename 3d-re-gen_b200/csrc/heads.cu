@@ -13,12 +13,6 @@ namespace {
 
 using namespace r3g;
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 constexpr int kRowsPerWarp = 4;
 constexpr int kMaxB = 8;
 
@@ -81,7 +75,7 @@ __global__ void __launch_bounds__(256) gemv_f32_kernel(const __half* __restrict_
     const int n = n0 + r;
 #pragma unroll
     for (int b = 0; b < BT; ++b) {
-      float v = warp_sum_f(acc[r][b]);
+      float v = warp_sum(acc[r][b]);
       if (lane == 0 && n < N && b < B) {
         if (bias) v += bias[n];
         if (act_out == 1) v = 0.5f * v * (1.f + erff(v * 0.7071067811865476f));
@@ -106,7 +100,7 @@ __global__ void __launch_bounds__(256) layernorm_f32_kernel(const float* __restr
   const float* xr = x + (int64_t)r * ldx;
   float s = 0.f;
   for (int i = threadIdx.x; i < width; i += blockDim.x) s += xr[i];
-  s = warp_sum_f(s);
+  s = warp_sum(s);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -121,7 +115,7 @@ __global__ void __launch_bounds__(256) layernorm_f32_kernel(const float* __restr
     const float d = xr[i] - mean;
     q += d * d;
   }
-  q = warp_sum_f(q);
+  q = warp_sum(q);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = q;
   __syncthreads();
@@ -165,7 +159,7 @@ __global__ void __launch_bounds__(128) small_attention_f32_kernel(const float* _
     float s = 0.f;
 #pragma unroll
     for (int d = 0; d < DPL; ++d) s = fmaf(qv[d], k[lane + 32 * d], s);
-    s = warp_sum_f(s) * scale;
+    s = warp_sum(s) * scale;
     const float mn = fmaxf(m, s), a = expf(m - mn), p = expf(s - mn);
     l = l * a + p;
 #pragma unroll
@@ -179,15 +173,12 @@ __global__ void __launch_bounds__(128) small_attention_f32_kernel(const float* _
 
 }  // namespace
 
-#define R3G_HEAD_GPU(ctx, name) \
-  if (!(ctx) || !(ctx)->encode_tiled) return r3g_fail((ctx), R3G_E_CUDA, name ": no CUDA device (there is no CPU fallback)"); \
-  r3g_device_guard r3g_guard_(ctx)
-
 extern "C" int r3g_gemv_f32(r3g_ctx* ctx, const void* w_f16, const float* bias, const float* vec, int64_t vec_ld, float* out,
                             int64_t out_ld, const float* residual, const float* gamma, int B, int N, int K, int act_in,
                             int act_out, void* stream) {
-  R3G_HEAD_GPU(ctx, "gemv_f32");
-  if (!w_f16 || !vec || !out || B < 1 || B > kMaxB || K % 8 || vec_ld % 4 || (((uintptr_t)w_f16) & 15) || (((uintptr_t)vec) & 15))
+  R3G_ENTRY(ctx, "gemv_f32");
+  if (!w_f16 || !vec || !out || B < 1 || B > kMaxB || K % 8 || vec_ld % 4 || !r3g_aligned16(w_f16) ||
+      !r3g_aligned16(vec))
     return r3g_fail(ctx, R3G_E_INVALID, "gemv_f32: B in [1,%d], K %% 8 == 0, 16-byte aligned w / vec required", kMaxB);
   const int bt = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
   const size_t smem = (size_t)bt * K * sizeof(float);
@@ -213,7 +204,7 @@ extern "C" int r3g_gemv_f32(r3g_ctx* ctx, const void* w_f16, const float* bias, 
 extern "C" int r3g_layernorm_f32(r3g_ctx* ctx, const float* x, int64_t ldx, float* y, int64_t ldy, int rows, int width,
                                  float eps, const float* w, const float* b, const float* shift, const float* scale,
                                  const float* gate, int64_t mod_ld, void* stream) {
-  R3G_HEAD_GPU(ctx, "layernorm_f32");
+  R3G_ENTRY(ctx, "layernorm_f32");
   if (!x || !y || width < 1 || ((shift == nullptr) != (scale == nullptr)) || ((gate == nullptr) != (scale == nullptr)))
     return r3g_fail(ctx, R3G_E_INVALID, "layernorm_f32: bad arguments (shift / scale / gate come together)");
   if (rows <= 0) return R3G_OK;
@@ -225,7 +216,7 @@ extern "C" int r3g_layernorm_f32(r3g_ctx* ctx, const float* x, int64_t ldx, floa
 
 extern "C" int r3g_small_attention_f32(r3g_ctx* ctx, const float* qkv, float* out, int B, int S, int H, int D, float scale,
                                        void* stream) {
-  R3G_HEAD_GPU(ctx, "small_attention_f32");
+  R3G_ENTRY(ctx, "small_attention_f32");
   if (!qkv || !out || B < 1 || S < 1 || S > 64 || H < 1 || D % 32 || D < 32 || D > 256)
     return r3g_fail(ctx, R3G_E_INVALID, "small_attention_f32: S <= 64 and D in {32, 64, ..., 256} required");
   const int warps = B * H * S;

@@ -688,9 +688,8 @@ extern "C" size_t r3g_mc_workspace_bytes(int n0, int n1, int n2) {
 
 extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, void* workspace,
                             size_t workspace_bytes, int64_t* nv_host, int64_t* nf_host, void* stream) {
-  if (!ctx || !grid || !nv_host || !nf_host) return r3g_fail(ctx, R3G_E_INVALID, "mc_count: null argument");
-  if (!ctx->encode_tiled) return r3g_fail(ctx, R3G_E_CUDA, "mc_count: no CUDA device (there is no CPU fallback)");
-  r3g_device_guard guard(ctx);
+  R3G_ENTRY(ctx, "mc_count");
+  if (!grid || !nv_host || !nf_host) return r3g_fail(ctx, R3G_E_INVALID, "mc_count: null argument");
   cudaStream_t s = (cudaStream_t)stream;
   McDims d;
   McWorkspace w;
@@ -698,7 +697,7 @@ extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int
   if (rc) return rc;
   rc = carve(ctx, d, workspace, workspace_bytes, w);
   if (rc) return rc;
-  if (((uintptr_t)grid & 15) == 0)     // 16-byte loads when the grid's base allows them
+  if (r3g_aligned16(grid))   // 16-byte loads when the grid's base allows them
     mc_bits_kernel<true><<<w.bits_grid, kThreads, 0, s>>>(grid, d.npts, level, w.bits, w.minmax);
   else
     mc_bits_kernel<false><<<w.bits_grid, kThreads, 0, s>>>(grid, d.npts, level, w.bits, w.minmax);
@@ -731,9 +730,8 @@ extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int
 extern "C" int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level,
                               const double* bounds_host, void* workspace, size_t workspace_bytes, float* verts,
                               int32_t* faces, void* stream) {
-  if (!ctx || !grid || !verts || !faces) return r3g_fail(ctx, R3G_E_INVALID, "mc_extract: null argument");
-  if (!ctx->encode_tiled) return r3g_fail(ctx, R3G_E_CUDA, "mc_extract: no CUDA device (there is no CPU fallback)");
-  r3g_device_guard guard(ctx);
+  R3G_ENTRY(ctx, "mc_extract");
+  if (!grid || !verts || !faces) return r3g_fail(ctx, R3G_E_INVALID, "mc_extract: null argument");
   cudaStream_t s = (cudaStream_t)stream;
   McDims d;
   McWorkspace w;
@@ -759,9 +757,8 @@ extern "C" int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, i
 
 extern "C" int r3g_mc_classify(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level,
                                unsigned char* case_out, void* stream) {
-  if (!ctx || !grid || !case_out) return r3g_fail(ctx, R3G_E_INVALID, "mc_classify: null argument");
-  if (!ctx->encode_tiled) return r3g_fail(ctx, R3G_E_CUDA, "mc_classify: no CUDA device (there is no CPU fallback)");
-  r3g_device_guard guard(ctx);
+  R3G_ENTRY(ctx, "mc_classify");
+  if (!grid || !case_out) return r3g_fail(ctx, R3G_E_INVALID, "mc_classify: null argument");
   McDims d;
   int rc = make_dims(ctx, n0, n1, n2, d);
   if (rc) return rc;

@@ -67,9 +67,7 @@ __global__ void uf_flatten_kernel(int* parent, int64_t nv) {
 
 extern "C" int r3g_mesh_components(r3g_ctx* ctx, const int32_t* faces, int64_t nf, int64_t nv, int32_t* labels,
                                    void* stream) {
-  if (!ctx || !ctx->encode_tiled)
-    return r3g_fail(ctx, R3G_E_CUDA, "mesh_components: no CUDA device (there is no CPU fallback)");
-  r3g_device_guard guard(ctx);
+  R3G_ENTRY(ctx, "mesh_components");
   if (!labels || (nf > 0 && !faces) || nv < 0 || nf < 0 || nv > 0x7fffffffLL)
     return r3g_fail(ctx, R3G_E_INVALID, "mesh_components: bad arguments");
   if (nv == 0) return R3G_OK;

@@ -54,6 +54,16 @@ static inline int r3g_fail(r3g_ctx* ctx, int code, const char* fmt, ...) {
   return code;
 }
 
+// First statement of every compute entry point: refuse a NULL or device-less context (there is no CPU fallback), then
+// make the context's device current for the rest of the call.  Argument checks come after it.
+#define R3G_ENTRY(ctx, name)                                                                           \
+  if (!(ctx) || !(ctx)->encode_tiled)                                                                  \
+    return r3g_fail((ctx), R3G_E_CUDA, name ": no CUDA device (there is no CPU fallback)");            \
+  r3g_device_guard r3g_guard_(ctx)
+
+// host-side test of the 16-byte alignment that 128-bit accesses and tensor-map bases need (a null pointer passes)
+static inline bool r3g_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 #define R3G_CUDA_OK(ctx, expr)                                                                         \
   do {                                                                                                 \
     cudaError_t _e = (expr);                                                                           \

@@ -1,5 +1,6 @@
-// Inline-PTX wrappers for the sm_90a primitives the kernels use: mbarrier, TMA (cp.async.bulk.tensor),
-// wgmma (warpgroup MMA, descriptors, fences), elect, cache hints.  No CUTLASS/CuTe dependency.
+// Device primitives shared by the kernels: inline-PTX wrappers for the sm_90a features (mbarrier, TMA
+// (cp.async.bulk.tensor), wgmma (warpgroup MMA, descriptors, fences), elect, cache hints, ex2.approx), warp reductions,
+// and the fp16 / fp32-pair packing helpers of the row kernels.  No CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -183,6 +184,17 @@ __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
   f2_unpack(a, a0, a1); f2_unpack(b, b0, b1);
   return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
+__device__ __forceinline__ uint32_t f2_to_h2(uint64_t v) {   // round a pair to packed fp16 (lo in the low half)
+  float lo, hi;
+  f2_unpack(v, lo, hi);
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ uint64_t h2_to_f2(uint32_t h) {
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return f2_pack(f.x, f.y);
+}
 
 // ----------------------------------------------------------------------------- wgmma descriptors
 // Shared-memory matrix descriptor (sm_90):
@@ -199,9 +211,48 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t sbo
   return d;
 }
 
+// ----------------------------------------------------------------------------- fp16
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ float h2f(__half h) { return __half2float(h); }
+__device__ __forceinline__ float rnd_h(float x) { return __half2float(__float2half_rn(x)); }
+
+// Eight halfs moved as ONE 128-bit access.  The payload is a uint4 on purpose: with `__half2 v[4]` the struct copy is
+// member-wise and nvcc emits four 32-bit LDG/STG per Half8 even under alignas(16) (found in the SASS by
+// tests/test_sass.py), i.e. four quarter-used sector requests per lane instead of one coalesced 16-byte one.
+struct alignas(16) Half8 {
+  uint4 u;
+};
+__device__ __forceinline__ void unpack8(const Half8 p, float* f) {   // by value: the caller's load stays one 128-bit access
+  const __half2* v = reinterpret_cast<const __half2*>(&p.u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float2 t = __half22float2(v[i]);
+    f[2 * i] = t.x;
+    f[2 * i + 1] = t.y;
+  }
+}
+__device__ __forceinline__ Half8 pack8(const float* f) {
+  Half8 p;
+  __half2* v = reinterpret_cast<__half2*>(&p.u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = __floats2half2_rn(f[2 * i], f[2 * i + 1]);
+  return p;
+}
+
+// ----------------------------------------------------------------------------- math
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// 2^x, MUFU approximation with denormals flushed to zero
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
 }
 
 }  // namespace r3g

@@ -4,46 +4,16 @@
 #include <cuda_fp16.h>
 #include <math.h>
 
+#include <type_traits>
+
 #include "r3g_internal.h"
 #include "r3g_ptx.cuh"
 
 using namespace r3g;
 
 namespace {
-// every fp16 row / vector these kernels touch moves as 16-byte accesses: pointers must be 16-byte aligned (leading
-// dimensions and column offsets are already required to be multiples of 8 halfs)
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float h2f(__half h) { return __half2float(h); }
-__device__ __forceinline__ float rnd_h(float x) { return __half2float(__float2half_rn(x)); }
-
-// Eight halfs moved as ONE 128-bit access.  The payload is a uint4 on purpose: with `__half2 v[4]` the struct copy is
-// member-wise and nvcc emits four 32-bit LDG/STG per Half8 even under alignas(16) (found in the SASS by
-// tests/test_sass.py), i.e. four quarter-used sector requests per lane instead of one coalesced 16-byte one.
-struct alignas(16) Half8 {
-  uint4 u;
-};
-__device__ __forceinline__ void unpack8(const Half8 p, float* f) {   // by value: the caller's load stays one 128-bit access
-  const __half2* v = reinterpret_cast<const __half2*>(&p.u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float2 t = __half22float2(v[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
-__device__ __forceinline__ Half8 pack8(const float* f) {
-  Half8 p;
-  __half2* v = reinterpret_cast<__half2*>(&p.u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = __floats2half2_rn(f[2 * i], f[2 * i + 1]);
-  return p;
-}
+// Every fp16 row / vector these kernels touch moves as 16-byte accesses: pointers must be 16-byte aligned (leading
+// dimensions and column offsets are already required to be multiples of 8 halfs).
 
 // ------------------------------------------------------------------------------------------- LayerNorm
 // One warp per row; the row (<= 2048 halfs) lives in registers between the statistics and the write.
@@ -54,18 +24,6 @@ constexpr int kLnMaxChunks = 8;  // 8 chunks * 32 lanes * 8 halfs = 2048
 // (4: width <= 1024, 8: width <= 2048).  The arithmetic works on fp32 pairs (f2_*, r3g_ptx.cuh) and the affine
 // weights sit in shared memory as fp32, which keeps the per-element instruction count low enough for an HBM-bound
 // fp16 LayerNorm.
-__device__ __forceinline__ uint32_t f2_to_h2(uint64_t v) {   // round a pair to packed fp16 (lo in the low half)
-  float lo, hi;
-  f2_unpack(v, lo, hi);
-  uint32_t r;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-__device__ __forceinline__ uint64_t h2_to_f2(uint32_t h) {
-  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
-  return f2_pack(f.x, f.y);
-}
-
 template <int NCH>
 __device__ __forceinline__ void load_row(Half8 (&d)[NCH], const Half8* xr, int lane, int nchunks) {
 #pragma unroll
@@ -196,6 +154,46 @@ __global__ void __launch_bounds__(256, NCH == 4 ? 3 : 2) layernorm_kernel(const 
 
 // ------------------------------------------------------------------------------------------- q/k norm
 // 8 lanes per 64-wide head, 4 (row, head, q|k) groups per warp.
+__device__ __forceinline__ float head_sum(float s) {   // over the 8 lanes of a head
+  s += __shfl_xor_sync(0xffffffffu, s, 1);
+  s += __shfl_xor_sync(0xffffffffu, s, 2);
+  s += __shfl_xor_sync(0xffffffffu, s, 4);
+  return s;
+}
+
+// Normalises in place the 8 features f this lane (sub = lane & 7) holds of a 64-wide head:
+//   rms:  f = fp16(f * rrms) * w            ((x*rrms).to(fp16) * scale)
+//   else: f = (f - mean) * rstd * w + b     (LayerNorm, b optional)
+__device__ __forceinline__ void norm_head8(float (&f)[8], bool rms, float eps, const __half* w, const __half* b,
+                                           int sub) {
+  float wf[8];
+  unpack8(reinterpret_cast<const Half8*>(w)[sub], wf);
+  if (rms) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s += f[i] * f[i];
+    const float rrms = rsqrtf(head_sum(s) * (1.f / 64.f) + eps);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) f[i] = rnd_h(f[i] * rrms) * wf[i];
+    return;
+  }
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) s += f[i];
+  const float mean = head_sum(s) * (1.f / 64.f);
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    float d = f[i] - mean;
+    q += d * d;
+  }
+  const float rstd = rsqrtf(head_sum(q) * (1.f / 64.f) + eps);
+  float bf[8];
+  if (b) unpack8(reinterpret_cast<const Half8*>(b)[sub], bf);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) f[i] = (f[i] - mean) * rstd * wf[i] + (b ? bf[i] : 0.f);
+}
+
 __global__ void __launch_bounds__(256) qk_norm_kernel(__half* __restrict__ buf, int64_t ld, int64_t ngroups,
                                                       int heads, int64_t q_off, int64_t k_off, int64_t head_stride,
                                                       int mode, float eps, const __half* __restrict__ q_w,
@@ -212,47 +210,10 @@ __global__ void __launch_bounds__(256) qk_norm_kernel(__half* __restrict__ buf, 
   int64_t row = rh / heads;
   if (seg_len > 0) row = (row / seg_len) * seg_stride + (row % seg_len);
   __half* p = buf + row * ld + (sel ? k_off : q_off) + (int64_t)h * head_stride + sub * 8;
-  const __half* wv = sel ? k_w : q_w;
-  const __half* bv = sel ? k_b : q_b;
   float f[8];
-  Half8 in = *reinterpret_cast<const Half8*>(p);
-  unpack8(in, f);
-  float o[8], wf[8];
-  unpack8(reinterpret_cast<const Half8*>(wv)[sub], wf);
-  if (mode == 0) {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s += f[i] * f[i];
-    s += __shfl_xor_sync(0xffffffffu, s, 1);
-    s += __shfl_xor_sync(0xffffffffu, s, 2);
-    s += __shfl_xor_sync(0xffffffffu, s, 4);
-    const float rrms = rsqrtf(s * (1.f / 64.f) + eps);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o[i] = rnd_h(f[i] * rrms) * wf[i];  // (x*rrms).to(fp16) * scale
-  } else {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s += f[i];
-    s += __shfl_xor_sync(0xffffffffu, s, 1);
-    s += __shfl_xor_sync(0xffffffffu, s, 2);
-    s += __shfl_xor_sync(0xffffffffu, s, 4);
-    const float mean = s * (1.f / 64.f);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      float d = f[i] - mean;
-      q += d * d;
-    }
-    q += __shfl_xor_sync(0xffffffffu, q, 1);
-    q += __shfl_xor_sync(0xffffffffu, q, 2);
-    q += __shfl_xor_sync(0xffffffffu, q, 4);
-    const float rstd = rsqrtf(q * (1.f / 64.f) + eps);
-    float bf[8];
-    if (bv) unpack8(reinterpret_cast<const Half8*>(bv)[sub], bf);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o[i] = (f[i] - mean) * rstd * wf[i] + (bv ? bf[i] : 0.f);
-  }
-  if (active) *reinterpret_cast<Half8*>(p) = pack8(o);
+  unpack8(*reinterpret_cast<const Half8*>(p), f);
+  norm_head8(f, mode == 0, eps, sel ? k_w : q_w, sel ? k_b : q_b, sub);
+  if (active) *reinterpret_cast<Half8*>(p) = pack8(f);
 }
 
 // ------------------------------------------------------------------------------------------- LayerNorm, fp32 input
@@ -333,31 +294,7 @@ __global__ void __launch_bounds__(256) qk_norm_rope_kernel(__half* __restrict__ 
   float f[8];
   unpack8(*reinterpret_cast<const Half8*>(p), f);
   const __half* wv = sel ? k_w : q_w;
-  const __half* bv = sel ? k_b : q_b;
-  if (wv) {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s += f[i];
-    s += __shfl_xor_sync(0xffffffffu, s, 1);
-    s += __shfl_xor_sync(0xffffffffu, s, 2);
-    s += __shfl_xor_sync(0xffffffffu, s, 4);
-    const float mean = s * (1.f / 64.f);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      float d = f[i] - mean;
-      q += d * d;
-    }
-    q += __shfl_xor_sync(0xffffffffu, q, 1);
-    q += __shfl_xor_sync(0xffffffffu, q, 2);
-    q += __shfl_xor_sync(0xffffffffu, q, 4);
-    const float rstd = rsqrtf(q * (1.f / 64.f) + eps);
-    float wf[8], bf[8];
-    unpack8(reinterpret_cast<const Half8*>(wv)[sub], wf);
-    if (bv) unpack8(reinterpret_cast<const Half8*>(bv)[sub], bf);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) f[i] = (f[i] - mean) * rstd * wf[i] + (bv ? bf[i] : 0.f);
-  }
+  if (wv) norm_head8(f, false, eps, wv, sel ? k_b : q_b, sub);
   float partner[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) partner[i] = __shfl_xor_sync(0xffffffffu, f[i], 2);
@@ -550,20 +487,14 @@ __global__ void __launch_bounds__(256) grid_fourier_kernel(__half* __restrict__ 
   fourier_row(o, out_ld, xh, gp.num_freqs, gp.include_pi);
 }
 
-__global__ void __launch_bounds__(256) points_fourier_kernel(const __half* __restrict__ q, __half* __restrict__ out,
+// T = __half or float queries
+template <typename T>
+__global__ void __launch_bounds__(256) points_fourier_kernel(const T* __restrict__ q, __half* __restrict__ out,
                                                              int64_t out_ld, int64_t n, int F, int include_pi) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  float xh[3] = {h2f(q[3 * i]), h2f(q[3 * i + 1]), h2f(q[3 * i + 2])};
-  fourier_row(out + i * out_ld, out_ld, xh, F, include_pi);
-}
-
-__global__ void __launch_bounds__(256) points_fourier_f32_kernel(const float* __restrict__ q, __half* __restrict__ out,
-                                                                 int64_t out_ld, int64_t n, int F, int include_pi) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float xh[3] = {q[3 * i], q[3 * i + 1], q[3 * i + 2]};
-  fourier_row<true>(out + i * out_ld, out_ld, xh, F, include_pi);
+  float xh[3] = {(float)q[3 * i], (float)q[3 * i + 1], (float)q[3 * i + 2]};
+  fourier_row<std::is_same<T, float>::value>(out + i * out_ld, out_ld, xh, F, include_pi);
 }
 
 template <bool kF32>
@@ -754,20 +685,17 @@ __global__ void __launch_bounds__(256) unproject_kernel(const float* __restrict_
 
 }  // namespace
 
-#define R3G_NEED_GPU(ctx, name) \
-  if (!(ctx) || !(ctx)->encode_tiled) return r3g_fail((ctx), R3G_E_CUDA, name ": no CUDA device (there is no CPU fallback)"); \
-  r3g_device_guard r3g_guard_(ctx)
-
 extern "C" int r3g_layernorm(r3g_ctx* ctx, const void* x, int64_t ldx, void* y, int64_t ldy, int rows, int width,
                              float eps, const void* w, const void* b, const void* scale, const void* shift,
                              int64_t mod_ld, int rows_per_batch, int seg_len, int64_t x_seg_stride,
                              int64_t y_seg_stride, void* stream) {
-  R3G_NEED_GPU(ctx, "layernorm");
+  R3G_ENTRY(ctx, "layernorm");
   if (width % 8 || width > kLnMaxChunks * 256 || ldx % 8 || ldy % 8 || (scale && (mod_ld % 8)))
     return r3g_fail(ctx, R3G_E_INVALID, "layernorm: width %d must be a multiple of 8 and <= %d", width,
                     kLnMaxChunks * 256);
   if ((scale == nullptr) != (shift == nullptr)) return r3g_fail(ctx, R3G_E_INVALID, "layernorm: scale/shift pair");
-  if (!aligned16(x) || !aligned16(y) || !aligned16(w) || !aligned16(b) || !aligned16(scale) || !aligned16(shift))
+  if (!r3g_aligned16(x) || !r3g_aligned16(y) || !r3g_aligned16(w) || !r3g_aligned16(b) || !r3g_aligned16(scale) ||
+      !r3g_aligned16(shift))
     return r3g_fail(ctx, R3G_E_INVALID, "layernorm: pointers must be 16-byte aligned");
   if (rows <= 0) return R3G_OK;
   // persistent beyond one resident wave (3 blocks per SM at width <= 1024, 2 above)
@@ -785,11 +713,11 @@ extern "C" int r3g_layernorm(r3g_ctx* ctx, const void* x, int64_t ldx, void* y, 
 
 extern "C" int r3g_layernorm_f32in(r3g_ctx* ctx, const float* x, int64_t ldx, void* y, int64_t ldy, int rows,
                                    int width, float eps, const void* w, const void* b, void* stream) {
-  R3G_NEED_GPU(ctx, "layernorm_f32in");
+  R3G_ENTRY(ctx, "layernorm_f32in");
   if (width % 8 || width > kLnMaxChunks * 256 || ldx % 4 || ldy % 8)
     return r3g_fail(ctx, R3G_E_INVALID, "layernorm_f32in: width %d must be a multiple of 8 and <= %d", width,
                     kLnMaxChunks * 256);
-  if (!aligned16(x) || !aligned16(y) || !aligned16(w) || !aligned16(b))
+  if (!r3g_aligned16(x) || !r3g_aligned16(y) || !r3g_aligned16(w) || !r3g_aligned16(b))
     return r3g_fail(ctx, R3G_E_INVALID, "layernorm_f32in: pointers must be 16-byte aligned");
   if (rows <= 0) return R3G_OK;
   layernorm_f32in_kernel<<<(rows + 7) / 8, 256, 0, (cudaStream_t)stream>>>(x, ldx, (__half*)y, ldy, rows, width, eps,
@@ -801,10 +729,10 @@ extern "C" int r3g_layernorm_f32in(r3g_ctx* ctx, const float* x, int64_t ldx, vo
 extern "C" int r3g_qk_norm_rope(r3g_ctx* ctx, void* qkv, int64_t ld, int64_t rows, int heads, float eps,
                                 const void* q_w, const void* q_b, const void* k_w, const void* k_b, float rope_freq,
                                 int tokens_per_frame, int n_special, int patches_w, void* stream) {
-  R3G_NEED_GPU(ctx, "qk_norm_rope");
+  R3G_ENTRY(ctx, "qk_norm_rope");
   if (ld % 8 || (q_w == nullptr) != (k_w == nullptr) || tokens_per_frame < 1 || patches_w < 1)
     return r3g_fail(ctx, R3G_E_INVALID, "qk_norm_rope: bad arguments");
-  if (!aligned16(qkv) || !aligned16(q_w) || !aligned16(q_b) || !aligned16(k_w) || !aligned16(k_b))
+  if (!r3g_aligned16(qkv) || !r3g_aligned16(q_w) || !r3g_aligned16(q_b) || !r3g_aligned16(k_w) || !r3g_aligned16(k_b))
     return r3g_fail(ctx, R3G_E_INVALID, "qk_norm_rope: pointers must be 16-byte aligned");
   const int64_t ngroups = rows * heads * 2;
   if (ngroups <= 0) return R3G_OK;
@@ -817,7 +745,7 @@ extern "C" int r3g_qk_norm_rope(r3g_ctx* ctx, void* qkv, int64_t ld, int64_t row
 
 extern "C" int r3g_patchify(r3g_ctx* ctx, const float* images, void* out, int64_t out_ld, int N, int H, int W,
                             int patch, const float* mean3_host, const float* std3_host, void* stream) {
-  R3G_NEED_GPU(ctx, "patchify");
+  R3G_ENTRY(ctx, "patchify");
   if (!images || !out || patch < 1 || H % patch || W % patch || out_ld < 3 * patch * patch)
     return r3g_fail(ctx, R3G_E_INVALID, "patchify: bad arguments");
   const float m[3] = {mean3_host ? mean3_host[0] : 0.f, mean3_host ? mean3_host[1] : 0.f, mean3_host ? mean3_host[2] : 0.f};
@@ -833,10 +761,10 @@ extern "C" int r3g_patchify(r3g_ctx* ctx, const float* images, void* out, int64_
 extern "C" int r3g_qk_norm(r3g_ctx* ctx, void* buf, int64_t ld, int rows, int heads, int64_t q_off, int64_t k_off,
                            int64_t head_stride, int mode, float eps, const void* q_w, const void* q_b,
                            const void* k_w, const void* k_b, int seg_len, int64_t seg_stride, void* stream) {
-  R3G_NEED_GPU(ctx, "qk_norm");
+  R3G_ENTRY(ctx, "qk_norm");
   if (ld % 8 || q_off % 8 || k_off % 8 || head_stride % 8 || !q_w)
     return r3g_fail(ctx, R3G_E_INVALID, "qk_norm: offsets/strides must be multiples of 8 halfs");
-  if (!aligned16(buf) || !aligned16(q_w) || !aligned16(q_b) || !aligned16(k_w) || !aligned16(k_b))
+  if (!r3g_aligned16(buf) || !r3g_aligned16(q_w) || !r3g_aligned16(q_b) || !r3g_aligned16(k_w) || !r3g_aligned16(k_b))
     return r3g_fail(ctx, R3G_E_INVALID, "qk_norm: pointers must be 16-byte aligned");
   const int nsel = k_w ? 2 : 1;
   const int64_t ngroups = (int64_t)rows * heads * nsel;
@@ -851,10 +779,10 @@ extern "C" int r3g_qk_norm(r3g_ctx* ctx, void* buf, int64_t ld, int rows, int he
 
 extern "C" int r3g_gemv(r3g_ctx* ctx, const void* w, const void* bias, const void* vec, int64_t vec_ld, void* out,
                         int64_t out_ld, int B, int N, int K, int silu_in, int silu_out, void* stream) {
-  R3G_NEED_GPU(ctx, "gemv");
+  R3G_ENTRY(ctx, "gemv");
   if (B < 1 || B > kGemvMaxB || K % 8 || vec_ld % 8)
     return r3g_fail(ctx, R3G_E_INVALID, "gemv: B in [1,%d], K %% 8 == 0 required", kGemvMaxB);
-  if (!aligned16(w)) return r3g_fail(ctx, R3G_E_INVALID, "gemv: the weight matrix must be 16-byte aligned");
+  if (!r3g_aligned16(w)) return r3g_fail(ctx, R3G_E_INVALID, "gemv: the weight matrix must be 16-byte aligned");
   const int bt = B <= 1 ? 1 : B <= 2 ? 2 : B <= 4 ? 4 : 8;
   const size_t smem = (size_t)bt * K * sizeof(float);
   if (smem > 48 * 1024) return r3g_fail(ctx, R3G_E_INVALID, "gemv: B_pad * K * 4 bytes must fit 48 KB of shared memory");
@@ -871,7 +799,7 @@ extern "C" int r3g_gemv(r3g_ctx* ctx, const void* w, const void* bias, const voi
 
 extern "C" int r3g_timestep_embedding(r3g_ctx* ctx, const void* t_f16, void* out, int B, int dim, float time_factor,
                                       float max_period, void* stream) {
-  R3G_NEED_GPU(ctx, "timestep_embedding");
+  R3G_ENTRY(ctx, "timestep_embedding");
   const int n = B * (dim / 2);
   timestep_embedding_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>((const __half*)t_f16, (__half*)out, B,
                                                                                  dim, time_factor, max_period);
@@ -881,7 +809,7 @@ extern "C" int r3g_timestep_embedding(r3g_ctx* ctx, const void* t_f16, void* out
 
 extern "C" int r3g_cfg_euler_step(r3g_ctx* ctx, void* x, const void* v, void* x_dup, int64_t n, float guidance,
                                   float dsigma, void* stream) {
-  R3G_NEED_GPU(ctx, "cfg_euler_step");
+  R3G_ENTRY(ctx, "cfg_euler_step");
   cfg_euler_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>((__half*)x, (const __half*)v,
                                                                                     (__half*)x_dup, n, guidance,
                                                                                     dsigma);
@@ -891,7 +819,7 @@ extern "C" int r3g_cfg_euler_step(r3g_ctx* ctx, void* x, const void* v, void* x_
 
 extern "C" int r3g_grid_fourier(r3g_ctx* ctx, void* out, int64_t out_ld, int64_t start, int64_t count, int R,
                                 const float* bounds6_host, int num_freqs, int include_pi, void* stream) {
-  R3G_NEED_GPU(ctx, "grid_fourier");
+  R3G_ENTRY(ctx, "grid_fourier");
   if (!bounds6_host || R < 1 || out_ld < 3 + 6 * num_freqs)
     return r3g_fail(ctx, R3G_E_INVALID, "grid_fourier: bad arguments");
   GridParams gp;
@@ -914,10 +842,10 @@ extern "C" int r3g_grid_fourier(r3g_ctx* ctx, void* out, int64_t out_ld, int64_t
 
 extern "C" int r3g_points_fourier(r3g_ctx* ctx, const void* queries, void* out, int64_t out_ld, int64_t n,
                                   int num_freqs, int include_pi, void* stream) {
-  R3G_NEED_GPU(ctx, "points_fourier");
+  R3G_ENTRY(ctx, "points_fourier");
   if (!queries || !out || out_ld < 3 + 6 * num_freqs) return r3g_fail(ctx, R3G_E_INVALID, "points_fourier: bad arguments");
   if (n <= 0) return R3G_OK;
-  points_fourier_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+  points_fourier_kernel<__half><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       (const __half*)queries, (__half*)out, out_ld, n, num_freqs, include_pi);
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;
@@ -925,8 +853,9 @@ extern "C" int r3g_points_fourier(r3g_ctx* ctx, const void* queries, void* out, 
 
 extern "C" int r3g_swiglu(r3g_ctx* ctx, const void* x, int64_t ldx, void* out, int64_t ldo, int64_t rows, int F,
                           void* stream) {
-  R3G_NEED_GPU(ctx, "swiglu");
-  if (!x || !out || F < 8 || F % 8 || ldx % 8 || ldo % 8 || ldx < 2 * (int64_t)F || ldo < F || !aligned16(x) || !aligned16(out))
+  R3G_ENTRY(ctx, "swiglu");
+  if (!x || !out || F < 8 || F % 8 || ldx % 8 || ldo % 8 || ldx < 2 * (int64_t)F || ldo < F || !r3g_aligned16(x) ||
+      !r3g_aligned16(out))
     return r3g_fail(ctx, R3G_E_INVALID, "swiglu: F %% 8 == 0, ldx >= 2F, 16-byte aligned rows required");
   if (rows <= 0) return R3G_OK;
   const int64_t total = rows * (F / 8);
@@ -939,11 +868,11 @@ extern "C" int r3g_swiglu(r3g_ctx* ctx, const void* x, int64_t ldx, void* out, i
 
 extern "C" int r3g_points_fourier_f32(r3g_ctx* ctx, const float* queries, void* out, int64_t out_ld, int64_t n,
                                       int num_freqs, int include_pi, void* stream) {
-  R3G_NEED_GPU(ctx, "points_fourier_f32");
+  R3G_ENTRY(ctx, "points_fourier_f32");
   if (!queries || !out || out_ld < 3 + 6 * num_freqs) return r3g_fail(ctx, R3G_E_INVALID, "points_fourier_f32: bad arguments");
   if (n <= 0) return R3G_OK;
-  points_fourier_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(queries, (__half*)out, out_ld, n,
-                                                                                             num_freqs, include_pi);
+  points_fourier_kernel<float><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      queries, (__half*)out, out_ld, n, num_freqs, include_pi);
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;
 }
@@ -951,9 +880,9 @@ extern "C" int r3g_points_fourier_f32(r3g_ctx* ctx, const float* queries, void* 
 extern "C" int r3g_lnpost_dot(r3g_ctx* ctx, const void* x, int64_t ldx, int rows, int width, float eps,
                               const void* ln_w, const void* ln_b, const void* w_out, const void* b_out, float* out,
                               void* stream) {
-  R3G_NEED_GPU(ctx, "lnpost_dot");
+  R3G_ENTRY(ctx, "lnpost_dot");
   if (width % 8 || width > kLnMaxChunks * 256 || ldx % 8) return r3g_fail(ctx, R3G_E_INVALID, "lnpost_dot: width");
-  if (!aligned16(x)) return r3g_fail(ctx, R3G_E_INVALID, "lnpost_dot: x must be 16-byte aligned");
+  if (!r3g_aligned16(x)) return r3g_fail(ctx, R3G_E_INVALID, "lnpost_dot: x must be 16-byte aligned");
   if (rows <= 0) return R3G_OK;
   const unsigned grid = (unsigned)min((rows + 7) / 8, ctx->num_sms * (width <= 1024 ? 3 : 2));
   auto go = [&](auto kern) {
@@ -968,7 +897,7 @@ extern "C" int r3g_lnpost_dot(r3g_ctx* ctx, const void* x, int64_t ldx, int rows
 
 extern "C" int r3g_unproject(r3g_ctx* ctx, const float* depth, const double* cam_to_world_host,
                              const float* intrinsic_host, void* out, int S, int H, int W, int out_f64, void* stream) {
-  R3G_NEED_GPU(ctx, "unproject");
+  R3G_ENTRY(ctx, "unproject");
   if (!depth || !cam_to_world_host || !intrinsic_host || !out || S < 1 || H < 1 || W < 1)
     return r3g_fail(ctx, R3G_E_INVALID, "unproject: bad arguments");
   const int64_t pairs = ((int64_t)H * W + 1) / 2;

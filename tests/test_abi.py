@@ -50,6 +50,28 @@ def test_compute_fails_loudly_without_gpu(lib):
     assert lib.r3g_version() >= 100
 
 
+def test_every_compute_call_refuses_a_context_without_device(lib):
+    """r3g_create(-1) returns R3G_E_CUDA but still hands back a (device-less) context, on any machine.  Every compute
+    entry point given that context, or a NULL one, returns R3G_E_CUDA before it reads an argument (all are zero / NULL
+    here), names itself in the error, and launches nothing."""
+    from r3g import _abi
+    not_compute = {"r3g_version", "r3g_create", "r3g_destroy", "r3g_last_error", "r3g_launch_count",
+                   "r3g_mc_workspace_bytes"}
+    calls = [(name, [t() for t in argtypes[1:]]) for name, (_, argtypes) in sorted(_abi.SIGNATURES.items())
+             if name not in not_compute]
+    assert len(calls) == 25
+    handle = ctypes.c_void_p()
+    assert lib.r3g_create(-1, ctypes.byref(handle)) == _abi.R3G_E_CUDA and handle
+    try:
+        for name, zeros in calls:
+            assert getattr(lib, name)(handle, *zeros) == _abi.R3G_E_CUDA, name
+            assert lib.r3g_last_error(handle).decode().startswith(name[len("r3g_"):] + ": no CUDA device"), name
+            assert getattr(lib, name)(None, *zeros) == _abi.R3G_E_CUDA, name
+        assert lib.r3g_launch_count(handle) == 0
+    finally:
+        lib.r3g_destroy(handle)
+
+
 def test_marching_cubes_workspace_size(lib):
     """r3g_mc_workspace_bytes is pure arithmetic (no device): it covers 16 B of vertex-id slots per grid point plus the
     sign bits, the crossed-cell list and the info words sized for every cell; degenerate grids give 0."""
