@@ -12,22 +12,14 @@ from . import _abi
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_RELU = 0, 1, 2, 3
 
 
-_call_device = None   # device of the op being issued (set by _ctx, read by _stream; contexts are not thread-safe)
-
-
 def _ctx(t):
-    """The r3g context of the tensor's device.  The library switches to that device for the duration of each call
-    (r3g_device_guard) and the launch goes to torch's current stream OF THAT DEVICE, so a pipeline on cuda:1 works
+    """The r3g context of the tensor's device and torch's current stream OF THAT DEVICE, which the launch goes to.  The
+    library switches to that device for the duration of each call (r3g_device_guard), so a pipeline on cuda:1 works
     without torch.cuda.set_device(1)."""
-    global _call_device
     if not t.is_cuda:
         raise RuntimeError("r3g ops need CUDA tensors: there is no CPU fallback")
-    _call_device = t.device.index if t.device.index is not None else torch.cuda.current_device()
-    return _abi.get_context(_call_device)
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream(_call_device).cuda_stream)
+    dev = t.device.index
+    return _abi.get_context(dev), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _p(t):
@@ -142,9 +134,9 @@ def linear(x, w, bias=None, **kw):
     qk_norm: dict(mode=QKN_RMS|QKN_LAYERNORM, q_col0, k_col0 (None: q only), cols, eps, q_w, q_b, k_w, k_b) -- the per-head
     q/k normalisation fused into the epilogue (see qkn_* in include/r3g.h).
     """
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     a, out, _keep = _linear_args(x, w, bias, **kw)
-    ctx.check(ctx.lib.r3g_linear(ctx.handle, C.byref(a), _stream()))
+    ctx.check(ctx.lib.r3g_linear(ctx.handle, C.byref(a), stream))
     return out
 
 
@@ -152,13 +144,13 @@ def linear_pair(first, second):
     """Two independent linears in ONE launch (r3g_linear_args.group_next): `first` / `second` are dicts of linear()'s
     arguments (x, w, bias, out, ...).  Results are those of linear(**first), linear(**second); the tiles of both problems
     share one persistent grid -- the img and txt streams of a DoubleStreamBlock fill the machine together."""
-    ctx = _ctx(first["x"])
+    ctx, stream = _ctx(first["x"])
     if second["x"].device != first["x"].device:
         raise ValueError("linear_pair: both problems must live on the same device")
     a, out_a, _ka = _linear_args(**first)
     b, out_b, _kb = _linear_args(**second)
     a.group_next = C.addressof(b)
-    ctx.check(ctx.lib.r3g_linear(ctx.handle, C.byref(a), _stream()))
+    ctx.check(ctx.lib.r3g_linear(ctx.handle, C.byref(a), stream))
     return out_a, out_b
 
 
@@ -169,7 +161,7 @@ def attention(q, k, v, out=None, scale=None):
         _f16(t, n)
         if t.dim() != 4 or t.shape[-1] != 64 or t.stride(-1) != 1:
             raise ValueError(f"{n} must be [B, L, H, 64] with unit inner stride")
-    ctx = _ctx(q)
+    ctx, stream = _ctx(q)
     B, Lq, H, _ = q.shape
     Lk = k.shape[1]
     if out is None:
@@ -181,7 +173,7 @@ def attention(q, k, v, out=None, scale=None):
     a.o, a.o_sb, a.o_sl, a.o_sh = out.data_ptr(), out.stride(0), out.stride(1), out.stride(2)
     a.B, a.H, a.Lq, a.Lk = B, H, Lq, Lk
     a.scale = float(scale if scale is not None else 64 ** -0.5)
-    ctx.check(ctx.lib.r3g_attention(ctx.handle, C.byref(a), _stream()))
+    ctx.check(ctx.lib.r3g_attention(ctx.handle, C.byref(a), stream))
     return out
 
 
@@ -189,7 +181,7 @@ def layernorm(x, weight=None, bias=None, eps=1e-6, scale=None, shift=None, rows_
     """LayerNorm over the last dim (+ optional (1+scale)*y+shift modulation with per-batch [B, width] vectors).
     x / out may be segmented views (see _rows)."""
     _f16(x, "x")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     x2, rows, width, ldx, xl, xst = _rows(x, "x")
     if out is None:
         out = torch.empty(x.shape, device=x.device, dtype=torch.float16)
@@ -200,7 +192,7 @@ def layernorm(x, weight=None, bias=None, eps=1e-6, scale=None, shift=None, rows_
     mod_ld = scale.stride(0) if scale is not None else 0
     ctx.check(ctx.lib.r3g_layernorm(ctx.handle, _p(x2), ldx, _p(o2), ldy, rows, width, float(eps), _p(weight),
                                     _p(bias), _p(scale), _p(shift), mod_ld, int(rows_per_batch), seg_len, xs, ys,
-                                    _stream()))
+                                    stream))
     return out
 
 
@@ -208,27 +200,27 @@ def layernorm_f32in(x, weight, bias, eps=1e-5, out=None):
     """LayerNorm of a float32 [rows, width] stream into fp16 (VGGT blocks keep the residual stream in fp32)."""
     if x.dtype != torch.float32 or not x.is_contiguous():
         raise TypeError("x must be contiguous float32")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     width = x.shape[-1]
     rows = x.numel() // width
     if out is None:
         out = torch.empty(x.shape, device=x.device, dtype=torch.float16)
     ctx.check(ctx.lib.r3g_layernorm_f32in(ctx.handle, _p(x), width, _p(out), out.stride(-2) if out.dim() > 1 else width,
-                                          rows, width, float(eps), _p(weight), _p(bias), _stream()))
+                                          rows, width, float(eps), _p(weight), _p(bias), stream))
     return out
 
 
 def qk_norm_rope_(qkv, heads, eps, q_w, q_b, k_w, k_b, rope_freq, tokens_per_frame, n_special, patches_w):
     """In place on a packed fp16 [rows, 3*H*64] (3,H,D) projection: q/k LayerNorm (if weights) + 2-D RoPE (if freq>0)."""
     _f16(qkv, "qkv")
-    ctx = _ctx(qkv)
+    ctx, stream = _ctx(qkv)
     if not qkv.is_contiguous():
         raise ValueError("qkv must be contiguous")
     ld = qkv.shape[-1]
     rows = qkv.numel() // ld
     ctx.check(ctx.lib.r3g_qk_norm_rope(ctx.handle, _p(qkv), ld, rows, heads, float(eps), _p(q_w), _p(q_b), _p(k_w),
                                        _p(k_b), float(rope_freq), int(tokens_per_frame), int(n_special),
-                                       int(patches_w), _stream()))
+                                       int(patches_w), stream))
     return qkv
 
 
@@ -237,7 +229,7 @@ def patchify(images, patch, mean=None, std=None, out_ld=None):
     if images.dtype != torch.float32 or images.dim() != 4 or images.shape[1] != 3:
         raise TypeError("images must be float32 [N,3,H,W]")
     images = images.contiguous()
-    ctx = _ctx(images)
+    ctx, stream = _ctx(images)
     N, _, H, W = images.shape
     kk = 3 * patch * patch
     out_ld = out_ld or ((kk + 7) // 8) * 8
@@ -245,7 +237,7 @@ def patchify(images, patch, mean=None, std=None, out_ld=None):
     m = (C.c_float * 3)(*(mean if mean is not None else (0.0, 0.0, 0.0)))
     sd = (C.c_float * 3)(*(std if std is not None else (1.0, 1.0, 1.0)))
     ctx.check(ctx.lib.r3g_patchify(ctx.handle, _p(images), _p(out), out_ld, N, H, W, int(patch), C.cast(m, C.c_void_p),
-                                   C.cast(sd, C.c_void_p), _stream()))
+                                   C.cast(sd, C.c_void_p), stream))
     return out
 
 
@@ -253,77 +245,77 @@ def qk_norm_(buf, heads, q_off, k_off, head_stride, mode, eps, q_w, q_b=None, k_
     """In-place per-head RMS (mode 0) / LayerNorm (mode 1) of q (and k) inside a packed buffer of rows
     ([rows, ld] or a segmented [S, L, ld] view)."""
     _f16(buf, "buf")
-    ctx = _ctx(buf)
+    ctx, stream = _ctx(buf)
     b2, rows, _, ld, sl, sst = _rows(buf, "buf")
     ctx.check(ctx.lib.r3g_qk_norm(ctx.handle, _p(b2), ld, rows, heads, q_off, k_off, head_stride, mode, float(eps),
-                                  _p(q_w), _p(q_b), _p(k_w), _p(k_b), sl, sst, _stream()))
+                                  _p(q_w), _p(q_b), _p(k_w), _p(k_b), sl, sst, stream))
     return buf
 
 
 def gemv(w, bias, vec, silu_in=False, silu_out=False, out=None):
     """out[b] = W . act(vec[b]) + bias for B <= 8 rows."""
     _f16(w, "w"); _f16(vec, "vec")
-    ctx = _ctx(vec)
+    ctx, stream = _ctx(vec)
     B, K = vec.shape
     N = w.shape[0]
     if out is None:
         out = torch.empty(B, N, device=vec.device, dtype=torch.float16)
     ctx.check(ctx.lib.r3g_gemv(ctx.handle, _p(w), _p(bias), _p(vec), vec.stride(0), _p(out), out.stride(0), B, N, K,
-                               int(silu_in), int(silu_out), _stream()))
+                               int(silu_in), int(silu_out), stream))
     return out
 
 
 def swiglu(x, F, out=None):
     """out[:, j] = silu(x[:, j]) * x[:, F + j]  (fp16 roundings of Dinov2SwiGLUFFN); x [M, 2F] -> out [M, F]."""
     _f16(x, "x")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     x2, rows, width, ldx, _, _ = _rows(x, "x")
     if width < 2 * F:
         raise ValueError("swiglu: x must hold 2F columns")
     if out is None:
         out = torch.empty(*x.shape[:-1], F, device=x.device, dtype=torch.float16)
     o2, orow, _, ldo, _, _ = _rows(out, "out")
-    ctx.check(ctx.lib.r3g_swiglu(ctx.handle, _p(x2), ldx, _p(o2), ldo, rows, int(F), _stream()))
+    ctx.check(ctx.lib.r3g_swiglu(ctx.handle, _p(x2), ldx, _p(o2), ldo, rows, int(F), stream))
     return out
 
 
 def timestep_embedding(t, dim=256, time_factor=1000.0, max_period=10000.0, out=None):
     _f16(t, "t")
-    ctx = _ctx(t)
+    ctx, stream = _ctx(t)
     if out is None:
         out = torch.empty(t.shape[0], dim, device=t.device, dtype=torch.float16)
     ctx.check(ctx.lib.r3g_timestep_embedding(ctx.handle, _p(t), _p(out), t.shape[0], dim, float(time_factor),
-                                             float(max_period), _stream()))
+                                             float(max_period), stream))
     return out
 
 
 def cfg_euler_step_(x, v, guidance, dsigma, x_dup=None):
     """x <- x + dsigma * (v_uncond + g (v_cond - v_uncond)); v = cat(cond, uncond)."""
     _f16(x, "x"); _f16(v, "v")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     n = x.numel()
     if v.numel() != 2 * n or not (x.is_contiguous() and v.is_contiguous()):
         raise ValueError("v must hold cond and uncond predictions, contiguous")
     ctx.check(ctx.lib.r3g_cfg_euler_step(ctx.handle, _p(x), _p(v), _p(x_dup), n, float(guidance), float(dsigma),
-                                         _stream()))
+                                         stream))
     return x
 
 
 def grid_fourier(out, start, count, R, bounds6, num_freqs, include_pi):
-    ctx = _ctx(out)
+    ctx, stream = _ctx(out)
     b = (C.c_float * 6)(*[float(v) for v in bounds6])
     ctx.check(ctx.lib.r3g_grid_fourier(ctx.handle, _p(out), out.stride(0), int(start), int(count), int(R),
-                                       C.cast(b, C.c_void_p), int(num_freqs), int(include_pi), _stream()))
+                                       C.cast(b, C.c_void_p), int(num_freqs), int(include_pi), stream))
     return out
 
 
 def points_fourier(queries, out, num_freqs, include_pi):
     """Fourier features of explicit fp16 query points [n, 3] -> out [n, >= 3+6F] (zero padded)."""
     _f16(queries, "queries")
-    ctx = _ctx(queries)
+    ctx, stream = _ctx(queries)
     q = queries.contiguous()
     ctx.check(ctx.lib.r3g_points_fourier(ctx.handle, _p(q), _p(out), out.stride(0), q.shape[0], int(num_freqs),
-                                         int(include_pi), _stream()))
+                                         int(include_pi), stream))
     return out
 
 
@@ -331,18 +323,18 @@ def points_fourier_f32(queries, out, num_freqs, include_pi):
     """Fourier features of explicit FLOAT32 query points [n, 3] (float32 arithmetic, fp16 result; FlashVDM levels)."""
     if queries.dtype != torch.float32:
         raise TypeError("queries must be float32")
-    ctx = _ctx(queries)
+    ctx, stream = _ctx(queries)
     q = queries.contiguous()
     ctx.check(ctx.lib.r3g_points_fourier_f32(ctx.handle, _p(q), _p(out), out.stride(0), q.shape[0], int(num_freqs),
-                                             int(include_pi), _stream()))
+                                             int(include_pi), stream))
     return out
 
 
 def lnpost_dot(x, ln_w, ln_b, w_out, b_out, out, eps=1e-5):
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     x2, rows, width, ldx, _, _ = _rows(x, "x")
     ctx.check(ctx.lib.r3g_lnpost_dot(ctx.handle, _p(x2), ldx, rows, width, float(eps), _p(ln_w), _p(ln_b), _p(w_out),
-                                     _p(b_out), _p(out), _stream()))
+                                     _p(b_out), _p(out), stream))
     return out
 
 
@@ -351,12 +343,12 @@ def im2col3x3(x, stride=1, relu_in=False, out=None):
     _f16(x, "x")
     if x.dim() != 4 or not x.is_contiguous():
         raise ValueError("im2col3x3: x must be a contiguous NHWC tensor")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     N, H, W, Cc = x.shape
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     if out is None:
         out = torch.empty(N * Ho * Wo, 9 * Cc, device=x.device, dtype=torch.float16)
-    ctx.check(ctx.lib.r3g_im2col3x3(ctx.handle, _p(x), _p(out), N, H, W, Cc, int(stride), int(relu_in), _stream()))
+    ctx.check(ctx.lib.r3g_im2col3x3(ctx.handle, _p(x), _p(out), N, H, W, Cc, int(stride), int(relu_in), stream))
     return out, Ho, Wo
 
 
@@ -365,11 +357,11 @@ def bilinear_nhwc(x, Ho, Wo, out=None):
     _f16(x, "x")
     if x.dim() != 4 or not x.is_contiguous():
         raise ValueError("bilinear_nhwc: x must be a contiguous NHWC tensor")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     N, Hi, Wi, Cc = x.shape
     if out is None:
         out = torch.empty(N, Ho, Wo, Cc, device=x.device, dtype=torch.float16)
-    ctx.check(ctx.lib.r3g_bilinear_nhwc(ctx.handle, _p(x), _p(out), N, Hi, Wi, int(Ho), int(Wo), Cc, _stream()))
+    ctx.check(ctx.lib.r3g_bilinear_nhwc(ctx.handle, _p(x), _p(out), N, Hi, Wi, int(Ho), int(Wo), Cc, stream))
     return out
 
 
@@ -384,7 +376,7 @@ def gemv_f32(w16, bias, vec, out=None, residual=None, gamma=None, silu_in=False,
     _f16(w16, "w")
     for t, n in ((bias, "bias"), (vec, "vec"), (residual, "residual"), (gamma, "gamma")):
         _f32(t, n)
-    ctx = _ctx(vec)
+    ctx, stream = _ctx(vec)
     B, K = vec.shape
     N = w16.shape[0]
     if out is None:
@@ -392,33 +384,33 @@ def gemv_f32(w16, bias, vec, out=None, residual=None, gamma=None, silu_in=False,
     if residual is not None and residual.stride(0) != out.stride(0):
         raise ValueError("gemv_f32: residual must share out's row stride")
     ctx.check(ctx.lib.r3g_gemv_f32(ctx.handle, _p(w16), _p(bias), _p(vec), vec.stride(0), _p(out), out.stride(0),
-                                   _p(residual), _p(gamma), B, N, K, int(silu_in), int(gelu_out), _stream()))
+                                   _p(residual), _p(gamma), B, N, K, int(silu_in), int(gelu_out), stream))
     return out
 
 
 def layernorm_f32(x, weight=None, bias=None, eps=1e-5, shift=None, scale=None, gate=None, out=None):
     """float32 LayerNorm over the last dim of [rows, width]; with shift / scale / gate: gate * (LN(x)(1+scale)+shift) + x."""
     _f32(x, "x")
-    ctx = _ctx(x)
+    ctx, stream = _ctx(x)
     rows, width = x.shape
     if out is None:
         out = torch.empty_like(x)
     mod_ld = scale.stride(0) if scale is not None else 0
     ctx.check(ctx.lib.r3g_layernorm_f32(ctx.handle, _p(x), x.stride(0), _p(out), out.stride(0), rows, width, float(eps),
                                         _p(_f32(weight, "weight")), _p(_f32(bias, "bias")), _p(_f32(shift, "shift")),
-                                        _p(_f32(scale, "scale")), _p(_f32(gate, "gate")), mod_ld, _stream()))
+                                        _p(_f32(scale, "scale")), _p(_f32(gate, "gate")), mod_ld, stream))
     return out
 
 
 def small_attention_f32(qkv, B, S, H, D, out=None):
     """qkv float32 [B*S, 3*H*D] laid out (3, H, D) -> [B*S, H*D]; softmax over the S tokens of each batch element."""
     _f32(qkv, "qkv")
-    ctx = _ctx(qkv)
+    ctx, stream = _ctx(qkv)
     if not qkv.is_contiguous() or qkv.shape != (B * S, 3 * H * D):
         raise ValueError("small_attention_f32: qkv must be contiguous [B*S, 3*H*D]")
     if out is None:
         out = torch.empty(B * S, H * D, device=qkv.device, dtype=torch.float32)
-    ctx.check(ctx.lib.r3g_small_attention_f32(ctx.handle, _p(qkv), _p(out), B, S, H, D, float(D) ** -0.5, _stream()))
+    ctx.check(ctx.lib.r3g_small_attention_f32(ctx.handle, _p(qkv), _p(out), B, S, H, D, float(D) ** -0.5, stream))
     return out
 
 
@@ -437,7 +429,7 @@ def closed_form_inverse_se3(se3):
 def unproject(depth, extrinsic, intrinsic, out_dtype=torch.float64, out=None):
     """depth: CUDA float32 [S,H,W]; extrinsic [S,3,4] / intrinsic [S,3,3]: host numpy float32 (cam from world).
     out: optional preallocated [S,H,W,3] tensor of `out_dtype` (a 1.6 GB float64 result is worth reusing)."""
-    ctx = _ctx(depth)
+    ctx, stream = _ctx(depth)
     S, H, W = depth.shape
     c2w = np.ascontiguousarray(closed_form_inverse_se3(np.asarray(extrinsic))[:, :3, :].astype(np.float64))
     k = np.ascontiguousarray(np.asarray(intrinsic, dtype=np.float32).reshape(S, 9))
@@ -447,7 +439,7 @@ def unproject(depth, extrinsic, intrinsic, out_dtype=torch.float64, out=None):
         raise ValueError("unproject: out must be a contiguous [S,H,W,3] tensor of out_dtype")
     ctx.check(ctx.lib.r3g_unproject(ctx.handle, _p(depth.contiguous()), c2w.ctypes.data_as(C.c_void_p),
                                     k.ctypes.data_as(C.c_void_p), _p(out), S, H, W,
-                                    1 if out_dtype == torch.float64 else 0, _stream()))
+                                    1 if out_dtype == torch.float64 else 0, stream))
     return out
 
 
@@ -474,7 +466,7 @@ def marching_cubes(grid, level=0.0, bounds=None):
     if grid.dtype != torch.float32 or grid.dim() != 3:
         raise TypeError("grid must be float32 [n0,n1,n2]")
     grid = grid.contiguous()
-    ctx = _ctx(grid)
+    ctx, stream = _ctx(grid)
     n0, n1, n2 = grid.shape
     ws_bytes = ctx.lib.r3g_mc_workspace_bytes(n0, n1, n2)
     dbg = os.environ.get("R3G_DEBUG_TIMING") == "1"
@@ -486,7 +478,7 @@ def marching_cubes(grid, level=0.0, bounds=None):
         t1 = time.perf_counter()
     nv, nf = C.c_int64(0), C.c_int64(0)
     rc = ctx.lib.r3g_mc_count(ctx.handle, _p(grid), n0, n1, n2, float(level), _p(ws), ws_bytes, C.byref(nv),
-                              C.byref(nf), _stream())
+                              C.byref(nf), stream)
     if rc == _abi.R3G_E_LEVEL:
         raise ValueError("Surface level must be within volume data range.")
     if rc == _abi.R3G_E_NOSURFACE:
@@ -508,7 +500,7 @@ def marching_cubes(grid, level=0.0, bounds=None):
         barr = (C.c_double * 6)(*[float(v) for v in bounds])
         bptr = C.cast(barr, C.c_void_p)
     ctx.check(ctx.lib.r3g_mc_extract(ctx.handle, _p(grid), n0, n1, n2, float(level), bptr, _p(ws), ws_bytes,
-                                     _p(verts), _p(faces), _stream()))
+                                     _p(verts), _p(faces), stream))
     if dbg:
         torch.cuda.synchronize()
         t4 = time.perf_counter()
@@ -521,17 +513,17 @@ def mesh_components(faces, num_vertices):
     """labels int32 [num_vertices]: the smallest vertex index of each vertex's connected component (see r3g.h)."""
     if faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
         raise TypeError("faces must be int32 [F, 3]")
-    ctx = _ctx(faces)
+    ctx, stream = _ctx(faces)
     f = faces.contiguous()
     labels = torch.empty(int(num_vertices), device=faces.device, dtype=torch.int32)
-    ctx.check(ctx.lib.r3g_mesh_components(ctx.handle, _p(f), f.shape[0], int(num_vertices), _p(labels), _stream()))
+    ctx.check(ctx.lib.r3g_mesh_components(ctx.handle, _p(f), f.shape[0], int(num_vertices), _p(labels), stream))
     return labels
 
 
 def mc_classify(grid, level=0.0):
     grid = grid.contiguous()
-    ctx = _ctx(grid)
+    ctx, stream = _ctx(grid)
     n0, n1, n2 = grid.shape
     out = torch.empty((n0 - 1) * (n1 - 1) * (n2 - 1), device=grid.device, dtype=torch.uint8)
-    ctx.check(ctx.lib.r3g_mc_classify(ctx.handle, _p(grid), n0, n1, n2, float(level), _p(out), _stream()))
+    ctx.check(ctx.lib.r3g_mc_classify(ctx.handle, _p(grid), n0, n1, n2, float(level), _p(out), stream))
     return out.view(n0 - 1, n1 - 1, n2 - 1)

@@ -19,6 +19,7 @@ import torch
 from . import ops
 from .conditioner import DinoImageEncoder, SingleImageEncoder
 from .dit import Hunyuan3DDiT
+from .graphs import GraphCache
 from .preprocessors import ImageProcessorV2
 from .scheduler import FlowMatchEulerDiscreteScheduler, FlowMatchEulerDiscreteSchedulerOutput
 from .vae import ShapeVAE, SurfaceExtractors
@@ -120,7 +121,7 @@ class Hunyuan3DDiTPipeline:
         self.device, self.dtype = torch.device(device), dtype
         self.kwargs = kwargs
         self.use_cuda_graph = True
-        self._graphs = {}
+        self._graphs = GraphCache(keep_all=True)
         self.replayed_launches = 0  # kernels executed through CUDA-graph replays (not seen by r3g_launch_count)
         self.timings = {}
 
@@ -296,40 +297,22 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         x = latents.contiguous()
         do_cfg = cond["main"].shape[0] == 2 * B
         x_in = torch.cat([x] * 2) if do_cfg else x
-        t_buf = torch.empty(x_in.shape[0], device=self.device, dtype=torch.float16)
+        t_buf = torch.full((x_in.shape[0],), 0.5, device=self.device, dtype=torch.float16)  # warm-up t; set per step
         ctx = {"main": cond["main"].contiguous()}
-        key = (x_in.shape, ctx["main"].shape)
-        graph = None
+        g = None
         if self.use_cuda_graph and self.model.taps is None:
-            g = self._graphs.get(key)
-            if g is None:
-                st = dict(x=x_in.clone(), t=t_buf.clone(), c=ctx["main"].clone())
-                side = torch.cuda.Stream()
-                side.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(side):
-                    st["x"].copy_(x_in); st["t"].fill_(0.5)
-                    self.model(st["x"], st["t"], {"main": st["c"]})  # warm-up: lazy attributes, workspaces
-                torch.cuda.current_stream().wait_stream(side)
-                from . import _abi
-                rctx = _abi.get_context(self.device.index or 0)
-                n0 = rctx.launches
-                cg = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(cg):
-                    st["v"] = self.model(st["x"], st["t"], {"main": st["c"]})
-                g = (cg, st, rctx.launches - n0)
-                self._graphs[key] = g
-            graph, st, n_kernels = g
-            st["c"].copy_(ctx["main"])
-            st["x"].copy_(x_in)
-            x_in = st["x"]
+            g = self._graphs.get((x_in.shape, ctx["main"].shape), (x_in, t_buf, ctx["main"]),
+                                 lambda xs, ts, cs: self.model(xs, ts, {"main": cs}))
+            g.inputs[0].copy_(x_in)
+            g.inputs[2].copy_(ctx["main"])
+            x_in, t_buf = g.inputs[:2]
         for i in range(n):
-            if graph is not None:
-                st["t"].copy_(t16[i].expand(x_in.shape[0]))
-                graph.replay()
-                self.replayed_launches += n_kernels
-                v = st["v"]
+            t_buf.copy_(t16[i].expand(x_in.shape[0]))
+            if g is not None:
+                g.replay()
+                self.replayed_launches += g.launches
+                v = g.outputs
             else:
-                t_buf.copy_(t16[i].expand(x_in.shape[0]))
                 v = self.model(x_in, t_buf, ctx)
             if do_cfg:
                 ops.cfg_euler_step_(x, v, guidance_scale, dsig[i], x_dup=x_in)

@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .graphs import GraphCache
 
 
 class Latent2MeshOutput:
@@ -48,7 +49,7 @@ class CrossAttentionDecoder:
         self.count = 0
         self.chunk_queries = 65536
         self.use_cuda_graph = True
-        self._graphs = {}
+        self._graphs = GraphCache()
         self.w = None
         self._ws = {}
 
@@ -124,8 +125,10 @@ class CrossAttentionDecoder:
         ops.lnpost_dot(x, w["ln_post.weight"], w["ln_post.bias"], w["output_proj.weight"], w["output_proj.bias"],
                        out_f32, eps=1e-5)
 
-    def _decode_grid_eager(self, latents, bounds6, R, flat):
+    def _decode_grid_eager(self, latents, bounds6, R, flat=None):
         total = (R + 1) ** 3
+        if flat is None:
+            flat = torch.empty(total, device=latents.device, dtype=torch.float32)
         cq = min(self.chunk_queries, total)
         ws = self._workspace(cq)
         kv = self._project_kv(latents)
@@ -133,38 +136,25 @@ class CrossAttentionDecoder:
             n = min(cq, total - s)
             ops.grid_fourier(ws["emb"][:n], s, n, R, bounds6, self.num_freqs, self.include_pi)
             self._decode(ws, n, kv, flat[s:s + n])
+        return flat
 
     def decode_grid(self, latents, bounds6, R, grid_out):
         """All (R+1)^3 dense-grid logits; queries are generated in-kernel (no [(R+1)^3, 3] list in HBM).
         The whole decode -- K/V projection + ceil((R+1)^3 / 65536) chunks x 10 kernels -- is captured ONCE per
         (R, bounds) into a CUDA graph over static buffers and replayed per object: eager launches left ~10 % of the
-        decode idle between kernels (tools/decode_probe.py: 2.61 ms per chunk in a graph, 2.90 ms eager)."""
+        decode idle between kernels (tools/decode_probe.py: 2.61 ms per chunk in a graph, 2.90 ms eager).
+        One (R, bounds) is cached at a time: the graph's grid is (R+1)^3 floats."""
         total = (R + 1) ** 3
         flat = grid_out.view(-1)
-        key = (int(R), tuple(float(b) for b in bounds6), tuple(latents.shape))
         if not self.use_cuda_graph or latents.device.type != "cuda":
             self._decode_grid_eager(latents, bounds6, R, flat)
         else:
-            g = self._graphs.get(key)
-            if g is None:
-                st = dict(lat=latents.clone(), grid=torch.empty(total, device=latents.device, dtype=torch.float32))
-                side = torch.cuda.Stream(latents.device)
-                side.wait_stream(torch.cuda.current_stream(latents.device))
-                with torch.cuda.stream(side):        # warm-up outside the capture: workspace, lazy function attributes
-                    n0 = min(self.chunk_queries, total)
-                    st["ws"] = self._workspace(n0)   # the graph keeps its workspace alive whatever _workspace caches later
-                    ops.grid_fourier(st["ws"]["emb"][:n0], 0, n0, R, bounds6, self.num_freqs, self.include_pi)
-                    self._decode(st["ws"], n0, self._project_kv(st["lat"]), st["grid"][:n0])
-                torch.cuda.current_stream(latents.device).wait_stream(side)
-                cg = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(cg):
-                    self._decode_grid_eager(st["lat"], bounds6, R, st["grid"])
-                g = (cg, st)
-                self._graphs = {key: g}             # one (R, bounds) at a time: the static grid is (R+1)^3 floats
-            cg, st = g
-            st["lat"].copy_(latents)
-            cg.replay()
-            flat.copy_(st["grid"])
+            key = (int(R), tuple(float(b) for b in bounds6), tuple(latents.shape))
+            g = self._graphs.get(key, (latents,), lambda lat: self._decode_grid_eager(lat, bounds6, R),
+                                 keep=self._workspace(min(self.chunk_queries, total)))
+            g.inputs[0].copy_(latents)
+            g.replay()
+            flat.copy_(g.outputs)
         self.count += total
         return grid_out
 

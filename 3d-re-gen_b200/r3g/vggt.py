@@ -17,6 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
+from .graphs import GraphCache
 
 _RESNET_MEAN = (0.485, 0.456, 0.406)
 _RESNET_STD = (0.229, 0.224, 0.225)
@@ -136,7 +137,7 @@ class Aggregator:
         self.device = torch.device(device)
         self._ws = {}
         self.use_cuda_graph = True
-        self._graphs = {}
+        self._graphs = GraphCache()
 
     def load_state_dict(self, sd, prefix=""):
         dev = self.device
@@ -157,7 +158,9 @@ class Aggregator:
         self.camera_token, self.register_token = _f(sd["camera_token"], dev), _f(sd["register_token"], dev)
         return self
 
-    def _workspace(self, rows):
+    def _workspace(self, shape):
+        B, S, _, H, W = shape
+        rows = B * S * ((H // self.patch_size) * (W // self.patch_size) + self.patch_start_idx)
         ws = self._ws.get(rows)
         if ws is None:
             e = lambda *s: torch.empty(*s, device=self.device, dtype=torch.float16)  # noqa: E731
@@ -180,24 +183,10 @@ class Aggregator:
         graph's static outputs -- valid until the next call with the same shape (`use_cuda_graph = False`: fresh ones)."""
         if not (self.use_cuda_graph and images.is_cuda):
             return self._forward(images)
-        key = tuple(images.shape)
-        g = self._graphs.get(key)
-        if g is None:
-            st = dict(x=images.clone())
-            side = torch.cuda.Stream(images.device)
-            side.wait_stream(torch.cuda.current_stream(images.device))
-            with torch.cuda.stream(side):
-                self._forward(st["x"])                   # warm-up: workspaces, lazily set function attributes
-            torch.cuda.current_stream(images.device).wait_stream(side)
-            cg = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(cg):
-                st["out"] = self._forward(st["x"])
-            g = (cg, st)
-            self._graphs = {key: g}
-        cg, st = g
-        st["x"].copy_(images)
-        cg.replay()
-        return st["out"]
+        g = self._graphs.get(tuple(images.shape), (images,), self._forward, keep=self._workspace(images.shape))
+        g.inputs[0].copy_(images)
+        g.replay()
+        return g.outputs
 
     def _forward(self, images):
         B, S, C_in, H, W = images.shape
@@ -206,7 +195,7 @@ class Aggregator:
         imgs = images.reshape(B * S, 3, H, W).float().contiguous()
         hp, wp = H // self.patch_size, W // self.patch_size
         P = hp * wp + self.patch_start_idx
-        ws = self._workspace(B * S * P)
+        ws = self._workspace(images.shape)
         if self.vit is None:
             cols = ops.patchify(imgs, self.patch_size, _RESNET_MEAN, _RESNET_STD, out_ld=self.kpad)
             patch = ops.linear(cols, self.pe_w, self.pe_b, out_dtype=torch.float32).view(B * S, hp * wp, self.dim)

@@ -13,6 +13,8 @@ S tokens only; DPT: ~0.4 TFLOP of cuDNN convolutions per frame).  They are expre
 import torch
 import torch.nn.functional as F
 
+from .graphs import GraphCache
+
 
 def quat_to_mat(q):
     """vggt/utils/rotation.py:14-44 -- scalar-last quaternion, un-normalised input allowed."""
@@ -100,7 +102,7 @@ class CameraHeadR3G:
                     for k, v in raw.items() if k.endswith(".weight") and v.dim() == 2 and v.shape[1] % 8 == 0}
         self.f32 = {k: v.to(device=dev, dtype=torch.float32).contiguous() for k, v in raw.items()}
         self.trunk_depth, self.heads, self.device = trunk_depth, num_heads, dev
-        self._graphs = {}
+        self._graphs = GraphCache()
         self.use_cuda_graph = True
 
     def _iterations(self, tokens, num_iterations):
@@ -137,24 +139,11 @@ class CameraHeadR3G:
         tokens = aggregated_tokens_list[-1][:, :, 0].float().contiguous()     # [B, S, 2C]: the camera token of the last layer
         if not self.use_cuda_graph:
             return self._iterations(tokens, num_iterations)
-        key = (tuple(tokens.shape), num_iterations)
-        g = self._graphs.get(key)
-        if g is None:
-            st = dict(x=tokens.clone())
-            side = torch.cuda.Stream(tokens.device)
-            side.wait_stream(torch.cuda.current_stream(tokens.device))
-            with torch.cuda.stream(side):
-                self._iterations(st["x"], num_iterations)
-            torch.cuda.current_stream(tokens.device).wait_stream(side)
-            cg = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(cg):
-                st["out"] = self._iterations(st["x"], num_iterations)
-            g = (cg, st)
-            self._graphs = {key: g}
-        cg, st = g
-        st["x"].copy_(tokens)
-        cg.replay()
-        return [o.clone() for o in st["out"]]
+        g = self._graphs.get((tuple(tokens.shape), num_iterations), (tokens,),
+                             lambda x: self._iterations(x, num_iterations))
+        g.inputs[0].copy_(tokens)
+        g.replay()
+        return [o.clone() for o in g.outputs]
 
 
 def _uv_embed(x, W, H, ratio=0.1):
@@ -312,7 +301,7 @@ class DPTHeadR3G:
         conv("scratch.output_conv2.0")
         conv("scratch.output_conv2.2")
         self.w = w
-        self._graphs, self._emb = {}, {}
+        self._graphs, self._emb = GraphCache(), {}
         self.use_cuda_graph = True
 
     # ---------------------------------------------------------------------------------------------- building blocks
@@ -402,25 +391,11 @@ class DPTHeadR3G:
         if not self.use_cuda_graph:
             pts, cf = self._impl(toks, H, W)
         else:
-            key = (B * S, H, W, toks[0].shape[-1])
-            g = self._graphs.get(key)
-            if g is None:
-                st = dict(x=[t.clone() for t in toks])
-                side = torch.cuda.Stream(self.device)
-                side.wait_stream(torch.cuda.current_stream(self.device))
-                with torch.cuda.stream(side):
-                    self._impl(st["x"], H, W)
-                torch.cuda.current_stream(self.device).wait_stream(side)
-                cg = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(cg):
-                    st["out"] = self._impl(st["x"], H, W)
-                g = (cg, st)
-                self._graphs = {key: g}
-            cg, st = g
-            for a, b in zip(st["x"], toks):
+            g = self._graphs.get((B * S, H, W, toks[0].shape[-1]), toks, lambda *x: self._impl(x, H, W))
+            for a, b in zip(g.inputs, toks):
                 a.copy_(b)
-            cg.replay()
-            pts, cf = (o.clone() for o in st["out"])
+            g.replay()
+            pts, cf = (o.clone() for o in g.outputs)
         return pts.view(B, S, *pts.shape[1:]), cf.view(B, S, *cf.shape[1:])
 
 

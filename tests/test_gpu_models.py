@@ -3,7 +3,9 @@
  (b) the fp32 oracle restatement run on the same device at the reference's full widths.
 Tolerances (stated, not bit-exact -- fp16 activations): relative L2 of hidden states <= 3e-3 per block tap,
 <= 1e-2 for the DiT output / SDF grid; SDF sign agreement reported separately."""
+import gc
 import os
+import weakref
 
 import numpy as np
 import pytest
@@ -82,9 +84,19 @@ def test_vae_and_sdf_grid_against_reference_fixture(golden_dir):
     assert (torch.sign(g[confident]) == torch.sign(gr[confident])).all()
     # explicit-query call form of the plug point
     q = torch.from_numpy(z["xyz"]).cuda().half()[None]
-    lg = vae.geo_decoder(queries=q, latents=lat_ref)
+    geo = vae.geo_decoder
+    captured = [weakref.ref(t) for t in next(iter(geo._ws.values())).values()]
+    lg = geo(queries=q, latents=lat_ref)
     assert lg.shape == (1, q.shape[1], 1)
     assert torch.equal(lg.view(-1).float().cpu(), g.view(-1))
+    # fewer queries size a smaller workspace, which replaces the one the grid's graph was captured with
+    geo(queries=q[:, :100], latents=lat_ref)
+    gc.collect()
+    assert all(r() is not None for r in captured), "the graph must keep its captured workspace alive"
+    again = vae.volume_decoder(lat_ref, geo, bounds=1.01, num_chunks=100, octree_resolution=Rr)
+    geo.use_cuda_graph = False
+    eager = vae.volume_decoder(lat_ref, geo, bounds=1.01, num_chunks=100, octree_resolution=Rr)
+    assert torch.equal(again, grid) and torch.equal(eager, grid), "graph replay must equal the eager launches"
 
 
 def test_sdf_decode_full_width_against_oracle():

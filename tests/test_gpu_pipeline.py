@@ -43,6 +43,33 @@ def test_denoise_loop_against_oracle_and_graph_equals_eager():
     assert torch.equal(again, outs[True])
 
 
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs a second GPU")
+def test_graphs_on_a_device_that_is_not_current():
+    """Models on cuda:1 with cuda:0 current: graph capture and replay follow the inputs' device."""
+    from r3g.pipelines import Hunyuan3DDiTFlowMatchingPipeline
+    from r3g.vggt_heads import CameraHeadR3G, random_state_dict
+    torch.cuda.set_device(0)
+    dev = torch.device("cuda:1")
+    sd = random_state_dict(7, embed_dim=128, depth=1, vit_depth=1, trunk_depth=2, features=32,
+                           out_channels=(32, 64, 128, 128), img_size=56)
+    head = CameraHeadR3G({k: v for k, v in sd.items() if k.startswith("camera_head.")}, trunk_depth=2, num_heads=2,
+                         device=dev)
+    toks = [torch.randn(1, 2, 7, 256, device=dev)]
+    graph = head(toks)
+    head.use_cuda_graph = False
+    assert all(torch.equal(a, b) for a, b in zip(graph, head(toks)))
+    pipe = Hunyuan3DDiTFlowMatchingPipeline.from_random(seed=11, config=MINI, conditioner=None, device=dev)
+    cond = {"main": torch.cat([torch.randn(1, 24, 96), torch.zeros(1, 24, 96)]).to(dev).half()}
+    lat0 = torch.randn((1, 48, 64), generator=torch.manual_seed(1234567), dtype=torch.float16)
+    outs = {}
+    for use_graph in (False, True):
+        pipe.use_cuda_graph = use_graph
+        outs[use_graph] = pipe(cond=cond, latents=lat0.clone(), num_inference_steps=6, guidance_scale=5.0,
+                               output_type="latent")
+    assert outs[True].device == dev and torch.equal(outs[False], outs[True])
+    assert torch.cuda.current_device() == 0
+
+
 def test_mesh_output_matches_cpu_marching_cubes_on_the_same_grid():
     import mc as omc
     pipe = make_pipe()

@@ -2,7 +2,9 @@
 by the reference's own Aggregator / DinoVisionTransformer modules, and at full width against the fp32 oracle.
 Tolerance: the reference itself runs this under bf16 autocast (8 mantissa bits); we require rel-L2 <= 5e-3
 against the fp32 ground truth."""
+import gc
 import os
+import weakref
 
 import numpy as np
 import pytest
@@ -43,11 +45,24 @@ def test_aggregator_and_dino_mini_against_reference_fixture(golden_dir):
     sd = {k[len("w:agg."):]: torch.from_numpy(z[k]) for k in z.files if k.startswith("w:agg.")}
     agg = Aggregator(img_size=56, patch_size=14, embed_dim=128, depth=2, num_heads=2, patch_embed="conv")
     agg.load_state_dict(sd)
-    outs, psi = agg(torch.from_numpy(z["agg_images"]).cuda())
+    images = torch.from_numpy(z["agg_images"]).cuda()
+    outs, psi = agg(images)
     assert psi == int(z["agg_psi"]) and len(outs) == 2
     for i, o in enumerate(outs):
         assert o.dtype == torch.float32 and tuple(o.shape) == z[f"agg_out{i}"].shape
         assert rel_l2(o, torch.from_numpy(z[f"agg_out{i}"])) < 5e-3
+    # graph replay == eager launches; the graph keeps its workspace when an eager call of another shape replaces it
+    graph_outs = [o.clone() for o in outs]
+    captured = [weakref.ref(t) for t in next(iter(agg._ws.values())).values()]
+    agg.use_cuda_graph = False
+    eager, _ = agg(images)
+    assert all(torch.equal(a, b) for a, b in zip(eager, graph_outs)), "graph replay must equal the eager launches"
+    agg(images[:, :1])
+    gc.collect()
+    assert all(r() is not None for r in captured), "the graph must keep its captured workspace alive"
+    agg.use_cuda_graph = True
+    again, _ = agg(images)
+    assert all(torch.equal(a, b) for a, b in zip(again, graph_outs))
     vsd = {k[len("w:vit."):]: torch.from_numpy(z[k]) for k in z.files if k.startswith("w:vit.")}
     vit = DinoVisionTransformer(vsd, "", 128, 2, 2, 14, 4, torch.device("cuda"))
     for tag in ("native", "interp"):
