@@ -4,7 +4,15 @@ The reference's only parallelism on this path is data-parallel over objects (src
 task i -> GPU i % num_devices through a process pool, results meet on disk).  Here rank r takes objects
 {i : i % world == r} of the sorted list and rank 0 -- which runs the downstream scene assembly
 (src/scene_reconstruction/run.py:62-76 reads <out>/3D/<name>/<name>.glb) -- receives every mesh over
-NCCL (NVLink / NVSwitch): one all_gather of the (V, F) counts, then one send/recv of a packed payload per rank.
+NCCL (NVLink / NVSwitch).  Every mesh travels as one fixed-capacity `pack_mesh` message, [nv, nf, 0, 0, verts...,
+faces...] as int32 words, with the capacity agreed across ranks, so rank 0 posts its receives without a size exchange:
+
+  * MeshBatchGatherer: each rank packs its meshes into a [steps, capacity] staging buffer and sends it to rank 0 in
+    one message at the end; rank 0 lands the used words through a two-slot pinned ring.  The stage-3 twin and
+    bench.py at N > 1 use it.
+  * MeshStreamGatherer: one message per rank and object on a side stream, under the next object's compute; rank 0
+    lands it through a pinned ring on a consumer thread.  bench.py's e2e arm uses it at N = 1.
+
 There is no compute kernel to fuse this with: the payload is a few MB per object, after the last kernel.
 """
 import torch
@@ -20,61 +28,23 @@ def shard_indices(n_items, rank=None, world=None):
     return list(range(rank, n_items, world))
 
 
-def _pack(meshes, device):
-    parts = []
-    for v, f in meshes:
-        parts.append(v.reshape(-1).contiguous().view(torch.int32))
-        parts.append(f.reshape(-1).to(torch.int32).contiguous())
-    if not parts:
-        return torch.empty(0, dtype=torch.int32, device=device)
-    return torch.cat(parts)
+def _world_rank():
+    return (dist.get_world_size(), dist.get_rank()) if dist.is_initialized() else (1, 0)
 
 
-def gather_meshes(meshes, to_host=False, max_objects=None):
-    """meshes: list of (verts float32 [V,3], faces int32 [F,3]) tensors on this rank's device.
-    Returns, on rank 0, the list of all ranks' meshes ordered by (rank, local index); [] elsewhere.
-    Works on NCCL (CUDA tensors) and on gloo (CPU tensors; used by the world_size-2 CPU tests)."""
-    if not dist.is_initialized() or dist.get_world_size() == 1:
-        return [(v.cpu(), f.cpu()) if to_host else (v, f) for v, f in meshes]
-    world, rank = dist.get_world_size(), dist.get_rank()
-    device = meshes[0][0].device if meshes else torch.device("cuda", torch.cuda.current_device()) \
-        if dist.get_backend() == "nccl" else torch.device("cpu")
-    n_local = torch.tensor([len(meshes)], dtype=torch.int64, device=device)
-    n_all = [torch.zeros_like(n_local) for _ in range(world)]
-    dist.all_gather(n_all, n_local)
-    n_max = max(int(t.item()) for t in n_all) if max_objects is None else max_objects
-    counts = torch.zeros(max(n_max, 1), 2, dtype=torch.int64, device=device)
-    for i, (v, f) in enumerate(meshes):
-        counts[i, 0], counts[i, 1] = v.shape[0], f.shape[0]
-    all_counts = [torch.zeros_like(counts) for _ in range(world)]
-    dist.all_gather(all_counts, counts)
-    payload = _pack(meshes, device)
-    out = []
-    if rank == 0:
-        bufs, ops_ = {}, []
-        for r in range(1, world):
-            n_int = int((all_counts[r][:, 0].sum() + all_counts[r][:, 1].sum()).item()) * 3
-            bufs[r] = torch.empty(n_int, dtype=torch.int32, device=device)
-            if n_int:
-                ops_.append(dist.P2POp(dist.irecv, bufs[r], r))
-        if ops_:
-            for w in dist.batch_isend_irecv(ops_):
-                w.wait()
-        bufs[0] = payload
-        for r in range(world):
-            off = 0
-            for i in range(int(n_all[r].item())):
-                nv, nf = int(all_counts[r][i, 0]), int(all_counts[r][i, 1])
-                v = bufs[r][off:off + 3 * nv].view(torch.float32).view(nv, 3)
-                off += 3 * nv
-                f = bufs[r][off:off + 3 * nf].view(nf, 3)
-                off += 3 * nf
-                out.append((v.cpu(), f.cpu()) if to_host else (v, f))
-    else:
-        if payload.numel():
-            for w in dist.batch_isend_irecv([dist.P2POp(dist.isend, payload, 0)]):
-                w.wait()
-    return out
+def _agree_max(world, device, *values):
+    """The element-wise maximum of `values` over all ranks, in one all_reduce.  Every rank must post the SAME message
+    size (an NCCL send / recv pair with different counts is undefined) while callers size from their own meshes."""
+    if world == 1:
+        return [int(x) for x in values]
+    t = torch.tensor([int(x) for x in values], dtype=torch.int64, device=device)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    return t.tolist()
+
+
+def _mesh_views(msg, nv, nf):
+    """(verts float32 [nv, 3], faces int32 [nf, 3]): views into a pack_mesh message."""
+    return msg[4:4 + 3 * nv].view(torch.float32).view(nv, 3), msg[4 + 3 * nv:4 + 3 * nv + 3 * nf].view(nf, 3)
 
 
 def pack_mesh(buf, verts, faces, cap_v, cap_f):
@@ -92,23 +62,20 @@ def pack_mesh(buf, verts, faces, cap_v, cap_f):
 
 
 class MeshBatchGatherer:
-    """Device-resident gather for a batch of K objects per rank with NO collective while the objects compute: every
-    finished mesh is packed into this rank's staging buffer [K, cap] (no allocator traffic), and `finish()` moves the
-    whole buffer to rank 0 in one NCCL message per peer.  A send / recv kernel that is resident while a persistent,
-    statically scheduled GEMM runs can hold one of its SMs until the peer arrives -- measured at N = 8 as ~0.15 s per
-    object when the per-object exchange of MeshStreamGatherer overlapped the next object -- so the device-resident arm of
-    bench.py keeps its NVLink traffic out of the compute phase."""
+    """Device-resident gather for a batch of objects per rank with NO collective while the objects compute: every
+    finished mesh is packed into this rank's staging buffer [steps, cap] (no allocator traffic), and `finish()` moves
+    the whole buffer to rank 0 in one NCCL message per peer.  `steps` and the capacities are agreed as the maxima over
+    the ranks, so each rank may submit its own number of meshes (up to the `steps` it passed).  A send / recv kernel
+    that is resident while a persistent, statically scheduled GEMM runs can hold one of its SMs until the peer arrives --
+    measured at N = 8 as ~0.15 s per object when the per-object exchange of MeshStreamGatherer overlapped the next
+    object -- so the device-resident arm of bench.py keeps its NVLink traffic out of the compute phase."""
 
     def __init__(self, cap_vertices, cap_faces, steps, device, to_host=False):
-        self.world = dist.get_world_size() if dist.is_initialized() else 1
-        self.rank = dist.get_rank() if dist.is_initialized() else 0
-        caps = torch.tensor([int(cap_vertices), int(cap_faces)], dtype=torch.int64, device=device)
-        if self.world > 1:
-            dist.all_reduce(caps, op=dist.ReduceOp.MAX)
-        self.cap_v, self.cap_f = int(caps[0]), int(caps[1])
+        self.world, self.rank = _world_rank()
+        self.cap_v, self.cap_f, self.steps = _agree_max(self.world, device, cap_vertices, cap_faces, steps)
         self.cap = 4 + 3 * self.cap_v + 3 * self.cap_f
-        self.stage = torch.empty(steps, self.cap, dtype=torch.int32, device=device)
-        self.stage[:, :4] = 0
+        self.stage = torch.empty(self.steps, self.cap, dtype=torch.int32, device=device)
+        self.stage[:, :4] = 0               # a row that is never submitted reads as an absent object
         self.k = 0
         # everything finish() needs exists before the first object: rank 0's receive buffers, the pinned ring, and the
         # NCCL point-to-point connections (a first send / recv to a peer sets the channel up; done here on 4 words)
@@ -119,7 +86,7 @@ class MeshBatchGatherer:
 
     def _exchange(self, words=None):
         """Every peer's staging buffer (or its first `words` words of the first mesh) -> rank 0's receive buffers."""
-        if self.world == 1:
+        if self.world == 1 or self.steps == 0:
             return
         cut = (lambda b: b.view(-1)[:words]) if words else (lambda b: b)
         if self.rank == 0:
@@ -135,9 +102,9 @@ class MeshBatchGatherer:
 
     def finish(self, to_host=False, sink=None):
         """Moves every rank's staging buffer to rank 0 (one NCCL message per peer).  Returns, on rank 0, the per-rank
-        buffers [world][K, cap] on the device; elsewhere [].  to_host: rank 0 then copies the USED words of every mesh
-        through a two-slot pinned ring (copy engine, large transfers) and calls sink(step, rank, verts, faces) with views
-        into the slot as each one lands."""
+        buffers [world][steps, cap] on the device; elsewhere [].  to_host: rank 0 then copies the USED words of every
+        mesh through a two-slot pinned ring (copy engine, large transfers) and calls sink(step, rank, verts, faces) with
+        views into the slot as each one lands; rows whose header reads nv == nf == 0 are skipped."""
         self._exchange()
         if self.rank != 0:
             return []
@@ -145,7 +112,7 @@ class MeshBatchGatherer:
         if not to_host:
             return bufs
         cuda = self.stage.is_cuda
-        hdr = torch.stack([b[:, :2] for b in bufs]).cpu()             # [world, K, 2]: nv, nf of every mesh
+        hdr = torch.stack([b[:, :2] for b in bufs]).cpu()             # [world, steps, 2]: nv, nf of every mesh
         ring = self.ring or [torch.empty(self.cap, dtype=torch.int32, pin_memory=cuda) for _ in range(2)]
         done = [None, None]
         pending = []
@@ -154,13 +121,14 @@ class MeshBatchGatherer:
             slot, r, k, nv, nf = item
             if done[slot] is not None:
                 done[slot].synchronize()
-            if sink is not None and (nv or nf):
-                src = ring[slot]
-                sink(k, r, src[4:4 + 3 * nv].view(torch.float32).view(nv, 3), src[4 + 3 * nv:4 + 3 * nv + 3 * nf].view(nf, 3))
+            if sink is not None:
+                sink(k, r, *_mesh_views(ring[slot], nv, nf))
         i = 0
         for r in range(len(bufs)):
-            for k in range(self.k):
+            for k in range(self.steps):
                 nv, nf = int(hdr[r, k, 0]), int(hdr[r, k, 1])
+                if nv == 0 and nf == 0:         # absent object, or a row its rank did not fill
+                    continue
                 slot = i % 2
                 if len(pending) == 2:           # the slot about to be overwritten must have been delivered
                     deliver(pending.pop(0))
@@ -195,19 +163,12 @@ class MeshStreamGatherer:
     def __init__(self, cap_vertices, cap_faces, device=None, to_host=True, depth=2, sink=None):
         import queue
         import threading
-        self.world = dist.get_world_size() if dist.is_initialized() else 1
-        self.rank = dist.get_rank() if dist.is_initialized() else 0
+        self.world, self.rank = _world_rank()
         self.cuda = torch.cuda.is_available() and (device is None or torch.device(device).type == "cuda") and (
             not dist.is_initialized() or dist.get_backend() == "nccl")
         self.device = torch.device(device) if device is not None else (
             torch.device("cuda", torch.cuda.current_device()) if self.cuda else torch.device("cpu"))
-        self.cap_v, self.cap_f = int(cap_vertices), int(cap_faces)
-        if self.world > 1:
-            # every rank must post the SAME message size (an NCCL send / recv pair with different counts is undefined);
-            # callers size the capacity from their own meshes, so agree on the maximum
-            caps = torch.tensor([self.cap_v, self.cap_f], dtype=torch.int64, device=self.device)
-            dist.all_reduce(caps, op=dist.ReduceOp.MAX)
-            self.cap_v, self.cap_f = int(caps[0]), int(caps[1])
+        self.cap_v, self.cap_f = _agree_max(self.world, self.device, cap_vertices, cap_faces)
         self.cap = 4 + 3 * self.cap_v + 3 * self.cap_f
         self.depth, self.to_host, self.step = depth, to_host, 0
         self.side = torch.cuda.Stream(self.device) if self.cuda else None
@@ -235,9 +196,6 @@ class MeshStreamGatherer:
         import contextlib
         return torch.cuda.stream(self.side) if self.cuda else contextlib.nullcontext()
 
-    def _pack(self, buf, verts, faces):
-        return pack_mesh(buf, verts, faces, self.cap_v, self.cap_f)
-
     def _consume(self):
         try:
             while True:
@@ -251,8 +209,7 @@ class MeshStreamGatherer:
                     if nv == 0 and nf == 0:
                         continue
                     src = self.land[slot][r] if self.to_host else (self.send[slot] if r == 0 else self.recv[slot][r - 1])
-                    v = src[4:4 + 3 * nv].view(torch.float32).view(nv, 3)      # views into the ring slot: a sink that
-                    f = src[4 + 3 * nv:4 + 3 * nv + 3 * nf].view(nf, 3)        # keeps them must copy before returning
+                    v, f = _mesh_views(src, nv, nf)     # views into the ring slot: a sink that keeps them must copy
                     if self.sink is not None:
                         self.sink(step, r, v, f)
                     else:
@@ -306,7 +263,7 @@ class MeshStreamGatherer:
         if self.cuda:
             if self._slot_done[slot] is not None:       # the slot's previous transfer / host copy must have left it
                 torch.cuda.current_stream(self.device).wait_event(self._slot_done[slot])
-        self._pack(self.send[slot], verts, faces)
+        pack_mesh(self.send[slot], verts, faces, self.cap_v, self.cap_f)
         if self.cuda:
             self.side.wait_stream(torch.cuda.current_stream(self.device))
         with self._stream():
@@ -332,7 +289,7 @@ class MeshStreamGatherer:
                 self._slot_done[slot].record(self.side)   # the send has left this slot
 
     def finish(self):
-        """Drain.  Returns, on rank 0, [(verts, faces)] ordered by (rank, step) -- gather_meshes' order; [] elsewhere."""
+        """Drain.  Returns, on rank 0, [(verts, faces)] ordered by (rank, step); [] elsewhere."""
         if self.rank != 0:
             if self.cuda:
                 self.side.synchronize()

@@ -9,7 +9,8 @@ mini, use_all_available_cuda; non-zero exit on failure.
 Differences, all on purpose:
   * one process per GPU (torchrun / torch.distributed, NCCL) instead of a spawn-pool that reloads both models for
     every image (reference run.py:108-133): each rank loads the weights once, takes images i % world == rank of
-    the SORTED list, and the finished meshes are gathered to rank 0 over NCCL, which writes every .glb;
+    the SORTED list, and the finished meshes are gathered to rank 0 (r3g/dist.py::MeshBatchGatherer, over NCCL
+    when there is more than one rank), which writes each .glb as its mesh lands;
   * FloaterRemover runs on the GPU (r3g/postprocessors.py: union-find components, MeshLab's 0.5 % rule) and
     DegenerateFaceRemover is the reference's no-op round trip; FaceReducer (pymeshlab quadric decimation to 40 000 faces)
     and the texture pipeline are not mirrored (SURVEY.md section 8f rows 2 and 4) -- the .glb holds the cleaned,
@@ -34,7 +35,7 @@ from PIL import Image
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
 
-from r3g.dist import gather_meshes, shard_indices  # noqa: E402
+from r3g.dist import MeshBatchGatherer, shard_indices  # noqa: E402
 from r3g.pipelines import Hunyuan3DDiTFlowMatchingPipeline, SimpleMesh  # noqa: E402
 from r3g.postprocessors import DegenerateFaceRemover, FloaterRemover  # noqa: E402
 
@@ -104,26 +105,31 @@ def main():
             v, f = torch.from_numpy(v), torch.from_numpy(f)
         # src/2d_to_3d_models/run.py:93-94 (FaceReducer, :95, is not mirrored)
         v, f = DegenerateFaceRemover()(FloaterRemover()((v, f), device=f"cuda:{local}"))
-        if world == 1:
-            v, f = v.cpu(), f.cpu()
         local_meshes.append((v, f))
         local_names.append(stem)
         print(f"[rank {rank}] {stem}: {v.shape[0]} vertices, {f.shape[0]} faces in {time.time() - t0:.2f} s", flush=True)
 
+    all_names = [local_names]
     if world > 1:
         all_names = [None] * world
         dist.all_gather_object(all_names, local_names)
-        meshes = gather_meshes(local_meshes, to_host=True)
-        ordered = [n for part in all_names for n in part]
-    else:
-        meshes, ordered = [(v.cpu(), f.cpu()) for v, f in local_meshes], local_names
+    gatherer = MeshBatchGatherer(max((v.shape[0] for v, _ in local_meshes), default=0),
+                                 max((f.shape[0] for _, f in local_meshes), default=0),
+                                 len(local_meshes), f"cuda:{local}", to_host=True)
+    for v, f in local_meshes:
+        gatherer.submit(v, f)
+    written = []
+
+    def write(k, r, v, f):              # v, f are views into the landing ring: used here, not kept
+        stem = all_names[r][k]
+        out_dir = os.path.join(output_folder, stem)
+        os.makedirs(out_dir, exist_ok=True)
+        # export_to_trimesh's winding flip (pipelines.py:102)
+        SimpleMesh(v.numpy(), f.numpy()[:, ::-1]).export(os.path.join(out_dir, f"{stem}.glb"))
+        written.append(stem)
+    gatherer.finish(to_host=True, sink=write)
     if rank == 0:
-        for stem, (v, f) in zip(ordered, meshes):
-            out_dir = os.path.join(output_folder, stem)
-            os.makedirs(out_dir, exist_ok=True)
-            # export_to_trimesh's winding flip (pipelines.py:102)
-            SimpleMesh(v.numpy(), f.numpy()[:, ::-1]).export(os.path.join(out_dir, f"{stem}.glb"))
-        print(f"wrote {len(meshes)} mesh(es) to {output_folder}")
+        print(f"wrote {len(written)} mesh(es) to {output_folder}")
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
