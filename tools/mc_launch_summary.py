@@ -13,7 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 
 KERNELS_PER_CALL = 8      # bits, mark, scan1, compact, eval, scan2, vertex, face
-CALLS_PER_VOLUME = 9      # warm-up + 7 timed + 1 with the phase print (tools/mc_probe.py)
+CALLS_PER_VOLUME = 8      # warm-up + 7 timed (tools/mc_probe.py)
 VOLUMES = ["257^3 torus", "257^3 dense", "513^3 torus", "513^3 dense"]
 
 

@@ -1,5 +1,5 @@
-"""Marching cubes by phase on the GPU: classify (+ scan + the 32-byte D2H of the totals) and the two emit passes, on a
-sparse surface (torus) and on a dense, noise-like one, at the metric's 257^3 and at 513^3.  Prints one JSON line.
+"""Whole-call marching-cubes timings on the GPU, on a sparse surface (torus) and on a dense, noise-like one, at the
+metric's 257^3 and at 513^3.  Prints one JSON line; tools/mc_launch_summary.py splits a call by kernel from an ncu run.
 
     python tools/mc_probe.py > gpurun_out/mc_probe.json
 """
@@ -39,9 +39,6 @@ def main():
                 torch.cuda.synchronize()
                 ts.append(1e3 * (time.perf_counter() - t0))
             ts.sort()
-            os.environ["R3G_DEBUG_TIMING"] = "1"
-            ops.marching_cubes(vol, 0.0)                # prints the phase split to stdout
-            os.environ.pop("R3G_DEBUG_TIMING")
             nbytes = n ** 3 * 4 + v.numel() * 4 + f.numel() * 4      # algorithmic: grid once + outputs once
             out.append(dict(n=n, volume=name, ms_median=ts[len(ts) // 2], ms_min=ts[0], verts=len(v), faces=len(f),
                             algorithmic_mb=nbytes / 1e6, gbs=nbytes / ts[len(ts) // 2] / 1e6))
