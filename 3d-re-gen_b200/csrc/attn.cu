@@ -36,7 +36,42 @@ struct AttnParams {
   int64_t o_sb, o_sh, o_sl;
   int Lq, Lk;
   float scale_log2;  // scale * log2(e)
+  // query windows (r3g_attention_args.win_*): nwin = 0, or one window per batch with the batches' query tiles
+  // concatenated along grid.x (window 1 from tile tiles0 on)
+  int nwin, tiles0;
+  int row0[2], len[2];
 };
+
+// The key/value fill of a windowed call: rows [dst0[b], dst0[b] + rows[b]) of k and v of batch b become copies of row
+// src[b] (r3g_attention_args.win_k0_count).
+struct KvFill {
+  __half *k, *v;
+  int64_t k_sb, k_sh, k_sl, v_sb, v_sh, v_sl;
+  int H;
+  int src[2], dst0[2], rows[2];
+};
+
+__global__ void __launch_bounds__(256) kv_fill_kernel(const KvFill f) {
+  pdl_wait();
+  pdl_trigger();
+  const int per_row = f.H * 2 * (kD / 8);           // 16-byte chunks of one row: heads x (k, v) x 8
+  const int64_t n0 = (int64_t)f.rows[0] * per_row, total = n0 + (int64_t)f.rows[1] * per_row;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int b = i >= n0;
+    int64_t r = b ? i - n0 : i;
+    const int c = (int)(r % (kD / 8));
+    r /= kD / 8;
+    const int kv = (int)(r & 1);
+    r >>= 1;
+    const int h = (int)(r % f.H);
+    r /= f.H;
+    __half* base = kv ? f.v : f.k;
+    const int64_t sb = kv ? f.v_sb : f.k_sb, sh = kv ? f.v_sh : f.k_sh, sl = kv ? f.v_sl : f.k_sl;
+    __half* head = base + b * sb + h * sh + 8 * c;
+    *reinterpret_cast<uint4*>(head + ((b ? f.dst0[1] : f.dst0[0]) + r) * sl) =
+        *reinterpret_cast<const uint4*>(head + (int64_t)(b ? f.src[1] : f.src[0]) * sl);
+  }
+}
 
 __global__ void __launch_bounds__(kThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
@@ -54,8 +89,15 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * kBQ;
-  const int h = blockIdx.y, b = blockIdx.z;
+  const int h = blockIdx.y;
+  int b = blockIdx.z, q0 = blockIdx.x * kBQ, row_base = 0, Lq = p.Lq;
+  if (p.nwin) {
+    const int w = blockIdx.x >= p.tiles0;
+    b = w;
+    q0 = (blockIdx.x - (w ? p.tiles0 : 0)) * kBQ;
+    row_base = w ? p.row0[1] : p.row0[0];
+    Lq = w ? p.len[1] : p.len[0];
+  }
   const int n_kv = (p.Lk + kBKV - 1) / kBKV;
 
   if (warp == 4 * kWG && lane == 0) {
@@ -79,9 +121,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
       // a warpgroup whose 64 rows all lie past Lq gets no Q (it computes on stale data and stores nothing)
-      const int groups = min(kWG, (p.Lq - q0 + 63) / 64);
+      const int groups = min(kWG, (Lq - q0 + 63) / 64);
       mbar_expect_tx(q_full, groups * kQBytes);
-      for (int g = 0; g < groups; ++g) tma_load_4d(sQ + g * kQBytes, &tmap_q, q_full, 0, q0 + 64 * g, h, b, kEvictFirst);
+      for (int g = 0; g < groups; ++g)
+        tma_load_4d(sQ + g * kQBytes, &tmap_q, q_full, 0, row_base + q0 + 64 * g, h, b, kEvictFirst);
       for (int j = 0; j < n_kv; ++j) {
         const int st = j % kStg;
         const uint32_t ph = (j / kStg) & 1;
@@ -177,8 +220,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
   for (int rr = 0; rr < 2; ++rr) {
     const int qrow = q0 + wg * 64 + r0 + 8 * rr;
-    if (qrow >= p.Lq) continue;
-    __half* op = p.o + (int64_t)b * p.o_sb + (int64_t)h * p.o_sh + (int64_t)qrow * p.o_sl;
+    if (qrow >= Lq) continue;
+    __half* op = p.o + (int64_t)b * p.o_sb + (int64_t)h * p.o_sh + (int64_t)(row_base + qrow) * p.o_sl;
 #pragma unroll
     for (int i = 2 * rr; i < kD / 2; i += 4)
       *reinterpret_cast<uint32_t*>(op + 8 * (i >> 2) + c0) = pack_half2(o[i] * inv_l[rr], o[i + 1] * inv_l[rr]);
@@ -206,17 +249,52 @@ extern "C" int r3g_attention(r3g_ctx* ctx, const r3g_attention_args* a, void* st
   if ((rc = make_qkv_map(ctx, &mq, a->q, a->q_sb, a->q_sh, a->q_sl, a->B, a->H, a->Lq, 64))) return rc;
   if ((rc = make_qkv_map(ctx, &mk, a->k, a->k_sb, a->k_sh, a->k_sl, a->B, a->H, a->Lk, kBKV))) return rc;
   if ((rc = make_qkv_map(ctx, &mv, a->v, a->v_sb, a->v_sh, a->v_sl, a->B, a->H, a->Lk, kBKV))) return rc;
-  AttnParams p;
+  AttnParams p = {};
   p.o = (__half*)a->o;
   p.o_sb = a->o_sb; p.o_sh = a->o_sh; p.o_sl = a->o_sl;
   p.Lq = a->Lq; p.Lk = a->Lk;
   p.scale_log2 = a->scale * 1.4426950408889634f;
+  int tiles = (a->Lq + kBQ - 1) / kBQ, grid_z = a->B;
+  KvFill f = {};
+  if (a->win_len[0] > 0) {
+    if (a->Lq != a->Lk || a->B > R3G_ATTN_MAX_WINDOWS)
+      return r3g_fail(ctx, R3G_E_INVALID, "attention: windows need Lq == Lk and B <= %d", R3G_ATTN_MAX_WINDOWS);
+    tiles = 0;
+    for (int w = 0; w < a->B; ++w) {
+      const int r0 = a->win_row0[w], n = a->win_len[w], cnt = a->win_k0_count[w] > 1 ? a->win_k0_count[w] : 1;
+      if (r0 < 0 || n < 1 || r0 + n > a->Lq || r0 - (cnt - 1) < 0)
+        return r3g_fail(ctx, R3G_E_INVALID, "attention: window %d [%d, %d + %d) with %d copies of its first key outside "
+                        "[0, %d)", w, r0, r0, n, cnt, a->Lq);
+      p.row0[w] = r0;
+      p.len[w] = n;
+      tiles += (n + kBQ - 1) / kBQ;
+      if (w == 0) p.tiles0 = tiles;
+      f.src[w] = r0;
+      f.dst0[w] = r0 - (cnt - 1);
+      f.rows[w] = cnt - 1;
+    }
+    p.nwin = a->B;
+    grid_z = 1;
+  }
+  if (f.rows[0] > 0 || f.rows[1] > 0) {
+    if (a->k_sb % 8 || a->k_sh % 8 || a->k_sl % 8 || a->v_sb % 8 || a->v_sh % 8 || a->v_sl % 8 || !r3g_aligned16(a->k) ||
+        !r3g_aligned16(a->v))
+      return r3g_fail(ctx, R3G_E_INVALID, "attention: copied keys need k / v strides that are multiples of 8 halfs");
+    f.k = (__half*)a->k; f.v = (__half*)a->v;
+    f.k_sb = a->k_sb; f.k_sh = a->k_sh; f.k_sl = a->k_sl;
+    f.v_sb = a->v_sb; f.v_sh = a->v_sh; f.v_sl = a->v_sl;
+    f.H = a->H;
+    const int64_t chunks = ((int64_t)f.rows[0] + f.rows[1]) * a->H * 2 * (kD / 8);
+    const unsigned fgrid = (unsigned)min((chunks + 255) / 256, (int64_t)ctx->num_sms * 8);
+    R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, kv_fill_kernel, dim3(fgrid), dim3(256), 0, (cudaStream_t)stream, f));
+    R3G_LAUNCH_OK(ctx);
+  }
   if (!(ctx->attr_done & R3G_ATTR_ATTENTION)) {   // function attributes are per device: one flag per context
     R3G_CUDA_OK(ctx, cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     R3G_CUDA_OK(ctx, cudaFuncSetAttribute(attention_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     ctx->attr_done |= R3G_ATTR_ATTENTION;
   }
-  dim3 grid((a->Lq + kBQ - 1) / kBQ, a->H, a->B);
+  dim3 grid(tiles, a->H, grid_z);
   R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, attention_kernel, grid, dim3(kThreads), kSmemBytes, (cudaStream_t)stream, mq, mk, mv, p));
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;

@@ -329,9 +329,12 @@ template <int BN>
 __global__ void __launch_bounds__(kNumThreads, Cfg<BN>::kMinBlocks)
 linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant__ CUtensorMap tmap_w0,
               const __grid_constant__ CUtensorMap tmap_x1, const __grid_constant__ CUtensorMap tmap_w1,
-              const __grid_constant__ LinearParams p0, const __grid_constant__ LinearParams p1) {
-  // Two problems may share one launch (r3g_linear_args.group_next: the img and txt streams of a DoubleStreamBlock):
-  // tiles [0, tiles0) belong to p0, the rest to p1 (p1.tiles_m == 0: no second problem).
+              const __grid_constant__ CUtensorMap tmap_x2, const __grid_constant__ CUtensorMap tmap_w2,
+              const __grid_constant__ LinearParams p0, const __grid_constant__ LinearParams p1,
+              const __grid_constant__ LinearParams p2) {
+  // Up to three problems share one launch (r3g_linear_args.group_next: the img and txt streams of a DoubleStreamBlock,
+  // the txt stream possibly split by batch): tiles [0, tiles0) belong to p0, [tiles0, tiles01) to p1, the rest to p2
+  // (tiles_m == 0: no such problem).
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atoms
@@ -344,17 +347,18 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int tiles0 = p0.tiles_m * p0.tiles_n;
+  const int tiles01 = tiles0 + p1.tiles_m * p1.tiles_n;
   const int tile = blockIdx.x;
-  const bool second = tile >= tiles0;
-  const LinearParams& p = second ? p1 : p0;
-  const int lt = second ? tile - tiles0 : tile;
+  const int which = tile >= tiles01 ? 2 : tile >= tiles0 ? 1 : 0;
+  const LinearParams& p = which == 2 ? p2 : which == 1 ? p1 : p0;
+  const int lt = tile - (which == 2 ? tiles01 : which == 1 ? tiles0 : 0);
   const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
   const int sg = tm / p.tiles_per_seg;
   const int num_k_blocks = (p.K + BK - 1) / BK;
 
   if (warp == kNumEpilogueWarps && lane == 0) {
-    tma_prefetch_desc(second ? &tmap_x1 : &tmap_x0);
-    tma_prefetch_desc(second ? &tmap_w1 : &tmap_w0);
+    tma_prefetch_desc(which == 2 ? &tmap_x2 : which == 1 ? &tmap_x1 : &tmap_x0);
+    tma_prefetch_desc(which == 2 ? &tmap_w2 : which == 1 ? &tmap_w1 : &tmap_w0);
     for (int s = 0; s < C::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 32 * kNumEpilogueWarps);   // every consumer thread releases the slot
@@ -367,8 +371,8 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
   if (warp == kNumEpilogueWarps) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      const CUtensorMap* tmap_x = second ? &tmap_x1 : &tmap_x0;
-      const CUtensorMap* tmap_w = second ? &tmap_w1 : &tmap_w0;
+      const CUtensorMap* tmap_x = which == 2 ? &tmap_x2 : which == 1 ? &tmap_x1 : &tmap_x0;
+      const CUtensorMap* tmap_w = which == 2 ? &tmap_w2 : which == 1 ? &tmap_w1 : &tmap_w0;
       const int l0 = (tm % p.tiles_per_seg) * BM;
       int stage = 0;
       uint32_t phase = 0;
@@ -479,7 +483,7 @@ struct Problem {
 int make_problem(r3g_ctx* ctx, const r3g_linear_args* a, int tile_m, int box_n, int bn, Problem& out) {
   LinearParams& p = out.p;
   memset(&p, 0, sizeof(p));
-  if (!a) return R3G_OK;   // no second problem: tiles_m = 0
+  if (!a) return R3G_OK;   // no such problem: tiles_m = 0
   const int seg_len = a->seg_len > 0 ? a->seg_len : a->M;
   const int nseg = a->M / seg_len;
   {
@@ -517,24 +521,28 @@ int make_problem(r3g_ctx* ctx, const r3g_linear_args* a, int tile_m, int box_n, 
   return R3G_OK;
 }
 
+constexpr int kMaxGroup = 3;   // problems per launch
+
+// probs[0..n): the non-empty problems of one call, n >= 1
 template <int BN>
-int launch_linear(r3g_ctx* ctx, const r3g_linear_args* a, const r3g_linear_args* b, cudaStream_t s) {
+int launch_linear(r3g_ctx* ctx, const r3g_linear_args* const* probs, int n, cudaStream_t s) {
   using C = Cfg<BN>;
-  Problem pa, pb;
-  int rc = make_problem(ctx, a, BM, BN, BN, pa);
-  if (rc) return rc;
-  rc = make_problem(ctx, b, BM, BN, BN, pb);
-  if (rc) return rc;
-  if (!b) { pb.tx = pa.tx; pb.tw = pa.tw; }
+  Problem pr[kMaxGroup];
+  int tiles = 0;
+  for (int i = 0; i < kMaxGroup; ++i) {
+    int rc = make_problem(ctx, i < n ? probs[i] : nullptr, BM, BN, BN, pr[i]);
+    if (rc) return rc;
+    if (i >= n) { pr[i].tx = pr[0].tx; pr[i].tw = pr[0].tw; }
+    tiles += pr[i].p.tiles_m * pr[i].p.tiles_n;
+  }
   constexpr unsigned kAttrBit = BN == 256 ? R3G_ATTR_LINEAR256 : R3G_ATTR_LINEAR128;
   if (!(ctx->attr_done & kAttrBit)) {
     R3G_CUDA_OK(ctx, cudaFuncSetAttribute(linear_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           C::kSmemBytes));
     ctx->attr_done |= kAttrBit;
   }
-  const int tiles = pa.p.tiles_m * pa.p.tiles_n + pb.p.tiles_m * pb.p.tiles_n;
-  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, linear_kernel<BN>, dim3(tiles), dim3(kNumThreads), C::kSmemBytes, s, pa.tx, pa.tw,
-                                   pb.tx, pb.tw, pa.p, pb.p));
+  R3G_CUDA_OK(ctx, r3g_launch_pdl(ctx, linear_kernel<BN>, dim3(tiles), dim3(kNumThreads), C::kSmemBytes, s, pr[0].tx,
+                                   pr[0].tw, pr[1].tx, pr[1].tw, pr[2].tx, pr[2].tw, pr[0].p, pr[1].p, pr[2].p));
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;
 }
@@ -571,16 +579,19 @@ int validate_linear(r3g_ctx* ctx, const r3g_linear_args* a) {
 extern "C" int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream) {
   R3G_ENTRY(ctx, "linear");
   if (!a) return r3g_fail(ctx, R3G_E_INVALID, "linear: null argument");
-  const r3g_linear_args* b = (const r3g_linear_args*)a->group_next;
-  if (b && b->group_next) return r3g_fail(ctx, R3G_E_INVALID, "linear: at most two problems per launch");
-  if (a->M <= 0) { a = b; b = nullptr; }
-  if (b && b->M <= 0) b = nullptr;
-  if (!a) return R3G_OK;
-  int rc = validate_linear(ctx, a);
-  if (rc) return rc;
-  if (b && (rc = validate_linear(ctx, b))) return rc;
+  // the non-empty problems of the group_next chain, in order
+  const r3g_linear_args* probs[kMaxGroup];
+  int n = 0, len = 0;
+  for (const r3g_linear_args* q = a; q; q = (const r3g_linear_args*)q->group_next) {
+    if (++len > kMaxGroup) return r3g_fail(ctx, R3G_E_INVALID, "linear: at most %d problems per launch", kMaxGroup);
+    if (q->M <= 0) continue;
+    int rc = validate_linear(ctx, q);
+    if (rc) return rc;
+    probs[n++] = q;
+  }
+  if (!n) return R3G_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  // Tile choice: wave efficiency (tiles / (waves * resident CTAs)) over the tiles of BOTH problems of a grouped launch.
+  // Tile choice: wave efficiency (tiles / (waves * resident CTAs)) over the tiles of ALL problems of a grouped launch.
   // A 128 x 256 tile reads half the operand bytes per FLOP of a 128 x 128 one but runs one CTA per SM instead of
   // two; it is taken unless it leaves more of the last wave idle.
   const int sms = ctx->num_sms;
@@ -590,13 +601,18 @@ extern "C" int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream) 
     return (double)tiles / (double)(waves * units);
   };
   auto tiles_of = [&](const r3g_linear_args* q, int tm, int tn) -> int64_t {
-    if (!q) return 0;
     const int seg = q->seg_len > 0 ? q->seg_len : q->M;
     return (int64_t)(q->M / seg) * ((seg + tm - 1) / tm) * ((q->N + tn - 1) / tn);
   };
-  const int n_min = b ? (a->N < b->N ? a->N : b->N) : a->N;
-  const double e256 = n_min >= 256 ? eff(tiles_of(a, BM, 256) + tiles_of(b, BM, 256), sms) : 0.0;
-  const double e128 = eff(tiles_of(a, BM, 128) + tiles_of(b, BM, 128), 2 * sms);
-  if (e256 > 0.0 && e256 >= e128) return launch_linear<256>(ctx, a, b, s);
-  return launch_linear<128>(ctx, a, b, s);
+  int n_min = probs[0]->N;
+  int64_t t256 = 0, t128 = 0;
+  for (int i = 0; i < n; ++i) {
+    n_min = probs[i]->N < n_min ? probs[i]->N : n_min;
+    t256 += tiles_of(probs[i], BM, 256);
+    t128 += tiles_of(probs[i], BM, 128);
+  }
+  const double e256 = n_min >= 256 ? eff(t256, sms) : 0.0;
+  const double e128 = eff(t128, 2 * sms);
+  if (e256 > 0.0 && e256 >= e128) return launch_linear<256>(ctx, probs, n, s);
+  return launch_linear<128>(ctx, probs, n, s);
 }

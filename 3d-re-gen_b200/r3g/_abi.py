@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libr3g.so")
 
 R3G_OK, R3G_E_INVALID, R3G_E_CUDA, R3G_E_WORKSPACE, R3G_E_LEVEL, R3G_E_NOSURFACE = 0, -1, -2, -3, -4, -5
+ATTN_MAX_WINDOWS = 2     # R3G_ATTN_MAX_WINDOWS
 
 
 class LinearArgs(C.Structure):
@@ -43,6 +44,8 @@ class AttentionArgs(C.Structure):
         ("o", C.c_void_p), ("o_sb", C.c_int64), ("o_sh", C.c_int64), ("o_sl", C.c_int64),
         ("B", C.c_int), ("H", C.c_int), ("Lq", C.c_int), ("Lk", C.c_int),
         ("scale", C.c_float),
+        ("win_row0", C.c_int * ATTN_MAX_WINDOWS), ("win_len", C.c_int * ATTN_MAX_WINDOWS),
+        ("win_k0_count", C.c_int * ATTN_MAX_WINDOWS),
     ]
 
 

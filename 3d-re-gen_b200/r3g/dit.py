@@ -171,8 +171,15 @@ class Hunyuan3DDiT:
         m = ws["mods"]
         return [m[:, off + i * H: off + (i + 1) * H] for i in range(n)]
 
-    def forward(self, x, t, contexts, **kwargs):
-        """x: [B, Li, in_channels] fp16, t: [B] fp16 in [0,1], contexts['main']: [B, Lt, context_in_dim] fp16."""
+    def forward(self, x, t, contexts, uncond_txt_shared=False, **kwargs):
+        """x: [B, Li, in_channels] fp16, t: [B] fp16 in [0,1], contexts['main']: [B, Lt, context_in_dim] fp16.
+
+        uncond_txt_shared: B == 2 (cond, uncond) and every text row of contexts['main'][1] is the same vector.  t is the
+        same for both samples too, so those Lt rows stay equal through every block (all ops but attention are
+        row-wise, and equal queries see equal keys): batch 1 then runs its GEMMs and attention queries on the window
+        [Lt - 1, L) of live rows -- one representative text row plus the latents.  Attention still sees all L keys:
+        r3g_attention copies the representative row's k / v over the other Lt - 1 text rows first.  Every row is
+        computed as on the full path, so the output is the same bit for bit."""
         if self.w is None:
             raise RuntimeError("Hunyuan3DDiT: no weights loaded")
         w = self.w
@@ -181,6 +188,8 @@ class Hunyuan3DDiT:
         Lt = cond.shape[1]
         L = Li + Lt
         H, Mh, nh = self.hidden_size, self.mlp_hidden, self.num_heads
+        if uncond_txt_shared and B != 2:
+            raise ValueError(f"uncond_txt_shared needs the (cond, uncond) batch of 2, got B = {B}")
         ws = self._workspace(B, Li, Lt)
         X, XM, QKV, HID, S1 = ws["X"], ws["XM"], ws["QKV"], ws["HID"], ws["S1"]
         txt, img = X[:, :Lt], X[:, Lt:]
@@ -195,38 +204,53 @@ class Hunyuan3DDiT:
 
         q4 = QKV.view(B, L, 3, nh, 64)
         streams = (("img", img, Lt, Li), ("txt", txt, 0, Lt))
-        # the two streams' projections apply different weights to different rows of the joint buffers: one launch per
-        # PAIR (ops.linear_pair), so that 6144 + 2740 rows share the persistent grid (include/r3g.h: group_next)
-        pair = ops.linear_pair if self.group_streams else (lambda a, b: (ops.linear(**a), ops.linear(**b)))
+        # the GEMM problems of a double block: (stream, batches, first row, rows).  Collapsed, batch 1's text is its
+        # representative row Lt - 1 alone (rows [0, Lt - 1) of batch 1 are dead: nothing whose output is used reads them,
+        # except their k / v, which attention fills with row Lt - 1's before it reads them)
+        if uncond_txt_shared:
+            probs = (("img", slice(None), Lt, Li), ("txt", slice(0, 1), 0, Lt), ("txt", slice(1, 2), Lt - 1, 1))
+            windows = ((0, L, 1), (Lt - 1, Li + 1, Lt))
+        else:
+            probs = (("img", slice(None), Lt, Li), ("txt", slice(None), 0, Lt))
+            windows = None
+        # the streams' projections apply different weights to different rows of the joint buffers: one launch per
+        # group (ops.linear_pair / linear_group), so that all rows share one grid (include/r3g.h: group_next)
+        if not self.group_streams:
+            group = lambda *ps: [ops.linear(**c) for c in ps]  # noqa: E731
+        else:
+            group = ops.linear_group if uncond_txt_shared else ops.linear_pair
         for i in range(self.depth):
             p = f"double_blocks.{i}."
-            calls = []
             for s, xs, ofs, Ls in streams:
                 sh1, sc1, g1, sh2, sc2, g2 = self._mod(ws, (i, s), 6)
-                xm = XM[:, ofs:ofs + Ls]
-                ops.layernorm(xs, eps=1e-6, scale=sc1, shift=sh1, rows_per_batch=Ls, out=xm)
+                ops.layernorm(xs, eps=1e-6, scale=sc1, shift=sh1, rows_per_batch=Ls, out=XM[:, ofs:ofs + Ls])
+            calls = []
+            for s, bs, ofs, n in probs:
                 qs, ks = w[p + f"{s}_attn.norm.query_norm.scale"], w[p + f"{s}_attn.norm.key_norm.scale"]
-                c = dict(x=xm, w=w[p + f"{s}_attn.qkv.weight"], bias=w[p + f"{s}_attn.qkv.bias"], out=QKV[:, ofs:ofs + Ls])
+                c = dict(x=XM[bs, ofs:ofs + n], w=w[p + f"{s}_attn.qkv.weight"], bias=w[p + f"{s}_attn.qkv.bias"],
+                         out=QKV[bs, ofs:ofs + n])
                 if self.fuse_qk_norm:
                     c["qk_norm"] = dict(mode=ops.QKN_RMS, q_col0=0, k_col0=H, cols=H, eps=1e-6, q_w=qs, k_w=ks)
                 calls.append(c)
-            pair(*calls)
+            group(*calls)
             if not self.fuse_qk_norm:
                 for s, xs, ofs, Ls in streams:
                     ops.qk_norm_(QKV[:, ofs:ofs + Ls], nh, 0, H, 64, 0, 1e-6, w[p + f"{s}_attn.norm.query_norm.scale"], None,
                                  w[p + f"{s}_attn.norm.key_norm.scale"], None)
-            ops.attention(q4[:, :, 0], q4[:, :, 1], q4[:, :, 2], out=q4[:, :, 0])  # joint txt+img attention
-            pair(*[dict(x=QKV[:, ofs:ofs + Ls, :H], w=w[p + f"{s}_attn.proj.weight"], bias=w[p + f"{s}_attn.proj.bias"],
-                        out=xs, gate=self._mod(ws, (i, s), 6)[2], gate_rows=Ls, residual=xs) for s, xs, ofs, Ls in streams])
+            # joint txt+img attention
+            ops.attention(q4[:, :, 0], q4[:, :, 1], q4[:, :, 2], out=q4[:, :, 0], windows=windows)
+            group(*[dict(x=QKV[bs, ofs:ofs + n, :H], w=w[p + f"{s}_attn.proj.weight"], bias=w[p + f"{s}_attn.proj.bias"],
+                         out=X[bs, ofs:ofs + n], gate=self._mod(ws, (i, s), 6)[2][bs], gate_rows=n,
+                         residual=X[bs, ofs:ofs + n]) for s, bs, ofs, n in probs])
             for s, xs, ofs, Ls in streams:
                 sh1, sc1, g1, sh2, sc2, g2 = self._mod(ws, (i, s), 6)
                 ops.layernorm(xs, eps=1e-6, scale=sc2, shift=sh2, rows_per_batch=Ls, out=XM[:, ofs:ofs + Ls])
-            pair(*[dict(x=XM[:, ofs:ofs + Ls], w=w[p + f"{s}_mlp.0.weight"], bias=w[p + f"{s}_mlp.0.bias"],
-                        out=HID[:, ofs:ofs + Ls], act=ops.ACT_GELU_TANH) for s, xs, ofs, Ls in streams])
-            pair(*[dict(x=HID[:, ofs:ofs + Ls], w=w[p + f"{s}_mlp.2.weight"], bias=w[p + f"{s}_mlp.2.bias"], out=xs,
-                        gate=self._mod(ws, (i, s), 6)[5], gate_rows=Ls, residual=xs) for s, xs, ofs, Ls in streams])
-            if self.taps is not None:
-                self.taps.append(X.clone())
+            group(*[dict(x=XM[bs, ofs:ofs + n], w=w[p + f"{s}_mlp.0.weight"], bias=w[p + f"{s}_mlp.0.bias"],
+                         out=HID[bs, ofs:ofs + n], act=ops.ACT_GELU_TANH) for s, bs, ofs, n in probs])
+            group(*[dict(x=HID[bs, ofs:ofs + n], w=w[p + f"{s}_mlp.2.weight"], bias=w[p + f"{s}_mlp.2.bias"],
+                         out=X[bs, ofs:ofs + n], gate=self._mod(ws, (i, s), 6)[5][bs], gate_rows=n,
+                         residual=X[bs, ofs:ofs + n]) for s, bs, ofs, n in probs])
+            self._tap(X, Lt, uncond_txt_shared)
 
         s1q = S1[:, :, :H].unflatten(-1, (nh, 64))
         s1k = S1[:, :, H + Mh:2 * H + Mh].unflatten(-1, (nh, 64))
@@ -236,19 +260,24 @@ class Hunyuan3DDiT:
             shift, scale, gate = self._mod(ws, ("s", i), 3)
             ops.layernorm(X, eps=1e-6, scale=scale, shift=shift, rows_per_batch=L, out=XM)
             qs, ks = w[p + "norm.query_norm.scale"], w[p + "norm.key_norm.scale"]
+            l1 = dict(w=w[p + "linear1.weight"], bias=w[p + "linear1.bias"], act=ops.ACT_GELU_TANH, act_cols=(H, H + Mh))
             if self.fuse_qk_norm:
-                ops.linear(XM, w[p + "linear1.weight"], w[p + "linear1.bias"], out=S1, act=ops.ACT_GELU_TANH,
-                           act_cols=(H, H + Mh),
-                           qk_norm=dict(mode=ops.QKN_RMS, q_col0=0, k_col0=H + Mh, cols=H, eps=1e-6, q_w=qs, k_w=ks))
+                l1["qk_norm"] = dict(mode=ops.QKN_RMS, q_col0=0, k_col0=H + Mh, cols=H, eps=1e-6, q_w=qs, k_w=ks)
+            l2 = dict(w=w[p + "linear2.weight"], bias=w[p + "linear2.bias"])
+            if uncond_txt_shared:   # batch 0's rows and batch 1's live window [Lt - 1, L), one launch each
+                ops.linear_pair(dict(x=XM[0], out=S1[0], **l1), dict(x=XM[1, Lt - 1:], out=S1[1, Lt - 1:], **l1))
             else:
-                ops.linear(XM, w[p + "linear1.weight"], w[p + "linear1.bias"], out=S1, act=ops.ACT_GELU_TANH,
-                           act_cols=(H, H + Mh))
+                ops.linear(XM, out=S1, **l1)
+            if not self.fuse_qk_norm:
                 ops.qk_norm_(S1, nh, 0, H + Mh, 64, 0, 1e-6, qs, None, ks, None)
-            ops.attention(s1q, s1k, s1v, out=s1q)
-            ops.linear(S1[:, :, :H + Mh], w[p + "linear2.weight"], w[p + "linear2.bias"], out=X, gate=gate,
-                       gate_rows=L, residual=X)
-            if self.taps is not None:
-                self.taps.append(X.clone())
+            ops.attention(s1q, s1k, s1v, out=s1q, windows=windows)
+            if uncond_txt_shared:
+                ops.linear_pair(dict(x=S1[0, :, :H + Mh], out=X[0], gate=gate[0:1], gate_rows=L, residual=X[0], **l2),
+                                dict(x=S1[1, Lt - 1:, :H + Mh], out=X[1, Lt - 1:], gate=gate[1:2], gate_rows=Li + 1,
+                                     residual=X[1, Lt - 1:], **l2))
+            else:
+                ops.linear(S1[:, :, :H + Mh], out=X, gate=gate, gate_rows=L, residual=X, **l2)
+            self._tap(X, Lt, uncond_txt_shared)
 
         shift, scale = self._mod(ws, "final", 2)
         xm = XM[:, Lt:]
@@ -258,6 +287,15 @@ class Hunyuan3DDiT:
         return out
 
     __call__ = forward
+
+    def _tap(self, X, Lt, uncond_txt_shared):
+        """Record the hidden state after a block (parity tests).  Collapsed, batch 1's dead text rows are given the value
+        of its representative row first, so that a tap means the same in both modes."""
+        if self.taps is None:
+            return
+        if uncond_txt_shared:
+            X[1, :Lt - 1] = X[1, Lt - 1:Lt]
+        self.taps.append(X.clone())
 
     # FLOPs of one forward for one sample (SURVEY.md section 8d): used by bench.py's roofline
     def flops_per_sample(self, Li, Lt):

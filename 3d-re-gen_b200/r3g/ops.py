@@ -174,21 +174,31 @@ def linear(x, w, bias=None, **kw):
     return out
 
 
+def linear_group(*problems):
+    """One to three independent linears in ONE launch (r3g_linear_args.group_next): each problem is a dict of linear()'s
+    arguments (x, w, bias, out, ...).  Results are those of linear(**p) for each p, returned in order; the tiles of all
+    problems share one grid -- the img and txt streams of a DoubleStreamBlock fill the machine together."""
+    if not 1 <= len(problems) <= 3:
+        raise ValueError(f"linear_group: 1 to 3 problems, got {len(problems)}")
+    dev = problems[0]["x"].get_device()
+    args, outs = zip(*[_linear_args(dev, **p) for p in problems])
+    for a, nxt in zip(args, args[1:]):
+        a.group_next = C.addressof(nxt)
+    _launch("linear", problems[0]["x"], C.byref(args[0]))
+    return outs
+
+
 def linear_pair(first, second):
-    """Two independent linears in ONE launch (r3g_linear_args.group_next): `first` / `second` are dicts of linear()'s
-    arguments (x, w, bias, out, ...).  Results are those of linear(**first), linear(**second); the tiles of both problems
-    share one persistent grid -- the img and txt streams of a DoubleStreamBlock fill the machine together."""
-    dev = first["x"].get_device()
-    a, out_a = _linear_args(dev, **first)
-    b, out_b = _linear_args(dev, **second)
-    a.group_next = C.addressof(b)
-    _launch("linear", first["x"], C.byref(a))
-    return out_a, out_b
+    """linear_group of two problems: the results of linear(**first), linear(**second) from one launch."""
+    return linear_group(first, second)
 
 
-def attention(q, k, v, out=None, scale=None):
+def attention(q, k, v, out=None, scale=None, windows=None):
     """softmax(q k^T * scale) v.  q: [B, Lq, H, 64] views (any strides with unit inner stride), k/v: [B, Lk, H, 64].
-    Returns/writes out: [B, Lq, H, 64] ("B L (H D)" when contiguous)."""
+    Returns/writes out: [B, Lq, H, 64] ("B L (H D)" when contiguous).
+    windows: None, or one (row0, length, k0_count) per batch (self-attention, B <= 2): batch b computes only the query
+    rows [row0, row0 + length), over all keys; rows of out outside a window are left as they were.  k0_count > 1 first
+    overwrites the k0_count - 1 rows of k and v before row0 with row0's k and v (see r3g_attention in r3g.h)."""
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _f16(t, n)
         if t.dim() != 4 or t.shape[-1] != 64 or t.stride(-1) != 1:
@@ -204,6 +214,11 @@ def attention(q, k, v, out=None, scale=None):
     a.o, a.o_sb, a.o_sl, a.o_sh = _ptr(out, dev, "attention", "out"), out.stride(0), out.stride(1), out.stride(2)
     a.B, a.H, a.Lq, a.Lk = B, H, Lq, Lk
     a.scale = float(scale if scale is not None else 64 ** -0.5)
+    if windows is not None:
+        if len(windows) != B:
+            raise ValueError(f"attention: {len(windows)} windows for {B} batches")
+        for b, (r0, n, cnt) in enumerate(windows):
+            a.win_row0[b], a.win_len[b], a.win_k0_count[b] = r0, n, cnt
     _launch("attention", q, C.byref(a))
     return out
 

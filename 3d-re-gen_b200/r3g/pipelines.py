@@ -299,10 +299,16 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         x_in = torch.cat([x] * 2) if do_cfg else x
         t_buf = torch.full((x_in.shape[0],), 0.5, device=self.device, dtype=torch.float16)  # warm-up t; set per step
         ctx = {"main": cond["main"].contiguous()}
+        # An unconditional context whose rows are all one vector (the zeros of unconditional_embedding) lets the DiT run
+        # that sample on one text row (Hunyuan3DDiT.forward: uncond_txt_shared).  Checked once per call: one sync.
+        shared = False
+        if do_cfg and B == 1:
+            un = ctx["main"][1]
+            shared = bool(torch.equal(un, un[:1].expand_as(un)))
         g = None
         if self.use_cuda_graph and self.model.taps is None:
-            g = self._graphs.get((x_in.shape, ctx["main"].shape), (x_in, t_buf, ctx["main"]),
-                                 lambda xs, ts, cs: self.model(xs, ts, {"main": cs}))
+            g = self._graphs.get((x_in.shape, ctx["main"].shape, shared), (x_in, t_buf, ctx["main"]),
+                                 lambda xs, ts, cs: self.model(xs, ts, {"main": cs}, uncond_txt_shared=shared))
             g.inputs[0].copy_(x_in)
             g.inputs[2].copy_(ctx["main"])
             x_in, t_buf = g.inputs[:2]
@@ -313,7 +319,7 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
                 self.replayed_launches += g.launches
                 v = g.outputs
             else:
-                v = self.model(x_in, t_buf, ctx)
+                v = self.model(x_in, t_buf, ctx, uncond_txt_shared=shared)
             if do_cfg:
                 ops.cfg_euler_step_(x, v, guidance_scale, dsig[i], x_dup=x_in)
             else:

@@ -101,10 +101,13 @@ int r3g_mesh_components(r3g_ctx* ctx, const int32_t* faces, int64_t nf, int64_t 
  *        [qkn_q_col0, qkn_q_col0 + qkn_cols) with (qkn_q_w, qkn_q_b) and, if qkn_k_col0 >= 0, of
  *        [qkn_k_col0, qkn_k_col0 + qkn_cols) with (qkn_k_w, qkn_k_b); the weights are fp16 [64] (bias NULL in mode 1).
  *        Column offsets and qkn_cols are multiples of 64; these columns must carry no activation / gate / residual.
- *   group_next: a second, independent problem (its own x / w / y / epilogue operands and sizes; its group_next must be
- *        NULL) whose tiles share this call's persistent grid.  The img and txt streams of a DoubleStreamBlock apply
- *        different weights to 6144 and 2740 rows (hunyuan3ddit.py:196-216): separately their N = 1024 projections
- *        fill 1.3 and 0.65 waves of 256 x 256 tiles, together 1.95 of 2.  Results are those of two separate calls.
+ *   group_next: a further, independent problem (its own x / w / y / epilogue operands and sizes) whose tiles share
+ *        this call's grid; a chain holds at most three problems (the third's group_next must be NULL).  The img and txt
+ *        streams of a DoubleStreamBlock apply different weights to 6144 and 2740 rows (hunyuan3ddit.py:196-216):
+ *        separately their N = 1024 projections fill 1.45 and 0.67 waves of 128 x 256 tiles on 132 SMs, together 2.1
+ *        of 3.  With the unconditional text collapsed to one row (r3g_attention windows) the txt stream is two
+ *        problems, batch 0's 1370 rows and batch 1's single row: img + both fill 240 of the 264 tiles of 2 waves.
+ *        Results are those of separate calls.
  */
 typedef struct {
   const void* x; int64_t ldx;
@@ -130,7 +133,16 @@ int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream);
  * hunyuan3ddit.py:33-36, attention_blocks.py:328, attention_processors.py:29-32, vggt/layers/attention.py:61).
  * head_dim is 64.  Q/K/V/O are addressed by strides in halfs: element (b, h, l, d) at
  * base + b*stride_b + h*stride_h + l*stride_l + d.  O has the "B L (H D)" layout of hunyuan3ddit.py:35 when
- * o_stride_l = H*64, o_stride_h = 64.  O may alias Q (each CTA reads its Q tile before writing it). */
+ * o_stride_l = H*64, o_stride_h = 64.  O may alias Q (each CTA reads its Q tile before writing it).
+ * Windows (self-attention only, Lq == Lk, B <= R3G_ATTN_MAX_WINDOWS): if win_len[0] > 0, batch b computes and writes
+ *   only the query rows [win_row0[b], win_row0[b] + win_len[b]) (the other rows of O are left as they are); every query
+ *   still attends all Lk keys.  If win_k0_count[b] = n > 1, the window's first row stands for n equal rows: the call
+ *   first overwrites rows [win_row0[b] - n + 1, win_row0[b]) of K and V with K and V of row win_row0[b] (in place, through
+ *   the k / v pointers), so the result is attention over n copies of that key, bit for bit.  The DiT's unconditional
+ *   CFG sample, whose Lt text rows are equal (hunyuan3ddit.py:33-36 with an all-equal text context), computes only its
+ *   last text row and the latents this way.  All batches share one launch.  Zeroed windows: plain attention over
+ *   [0, Lq). */
+#define R3G_ATTN_MAX_WINDOWS 2
 typedef struct {
   const void* q; int64_t q_sb, q_sh, q_sl;
   const void* k; int64_t k_sb, k_sh, k_sl;
@@ -138,6 +150,7 @@ typedef struct {
   void* o; int64_t o_sb, o_sh, o_sl;
   int B, H, Lq, Lk;
   float scale;
+  int win_row0[R3G_ATTN_MAX_WINDOWS], win_len[R3G_ATTN_MAX_WINDOWS], win_k0_count[R3G_ATTN_MAX_WINDOWS];
 } r3g_attention_args;
 int r3g_attention(r3g_ctx* ctx, const r3g_attention_args* a, void* stream);
 
