@@ -36,10 +36,11 @@ __global__ void uf_init_kernel(int* __restrict__ parent, int64_t nv) {
 }
 
 __global__ void uf_hook_kernel(int* parent, const int32_t* __restrict__ faces, int64_t nf, int64_t nv,
-                               int* __restrict__ bad) {
+                               int* __restrict__ bad, bool skip_dead) {
   const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= nf) return;
   const int a = faces[3 * f], b = faces[3 * f + 1], c = faces[3 * f + 2];
+  if (skip_dead && a < 0) return;
   if (a < 0 || b < 0 || c < 0 || a >= nv || b >= nv || c >= nv) {
     atomicExch(bad, 1);
     return;
@@ -65,6 +66,21 @@ __global__ void uf_flatten_kernel(int* parent, int64_t nv) {
 
 }  // namespace
 
+int r3g_launch_components(r3g_ctx* ctx, const int32_t* faces, int64_t nf, int64_t nv, int32_t* labels, int* bad_dev,
+                          bool skip_dead, cudaStream_t s) {
+  // labels doubles as the parent array (int32 [nv])
+  int* parent = reinterpret_cast<int*>(labels);
+  uf_init_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(parent, nv);
+  R3G_LAUNCH_OK(ctx);
+  if (nf > 0) {
+    uf_hook_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, s>>>(parent, faces, nf, nv, bad_dev, skip_dead);
+    R3G_LAUNCH_OK(ctx);
+  }
+  uf_flatten_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(parent, nv);
+  R3G_LAUNCH_OK(ctx);
+  return R3G_OK;
+}
+
 extern "C" int r3g_mesh_components(r3g_ctx* ctx, const int32_t* faces, int64_t nf, int64_t nv, int32_t* labels,
                                    void* stream) {
   R3G_ENTRY(ctx, "mesh_components");
@@ -72,19 +88,11 @@ extern "C" int r3g_mesh_components(r3g_ctx* ctx, const int32_t* faces, int64_t n
     return r3g_fail(ctx, R3G_E_INVALID, "mesh_components: bad arguments");
   if (nv == 0) return R3G_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  // labels doubles as the parent array (int32 [nv]); the flag lives in the context's pinned scratch
-  int* parent = reinterpret_cast<int*>(labels);
+  // the out-of-range flag is read back through the context's pinned scratch
   int* bad_dev = nullptr;
   R3G_CUDA_OK(ctx, cudaMallocAsync((void**)&bad_dev, sizeof(int), s));
   R3G_CUDA_OK(ctx, cudaMemsetAsync(bad_dev, 0, sizeof(int), s));
-  uf_init_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(parent, nv);
-  R3G_LAUNCH_OK(ctx);
-  if (nf > 0) {
-    uf_hook_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, s>>>(parent, faces, nf, nv, bad_dev);
-    R3G_LAUNCH_OK(ctx);
-  }
-  uf_flatten_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(parent, nv);
-  R3G_LAUNCH_OK(ctx);
+  if (int rc = r3g_launch_components(ctx, faces, nf, nv, labels, bad_dev, false, s)) return rc;
   int* bad_host = reinterpret_cast<int*>(ctx->pinned);
   R3G_CUDA_OK(ctx, cudaMemcpyAsync(bad_host, bad_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
   R3G_CUDA_OK(ctx, cudaFreeAsync(bad_dev, s));

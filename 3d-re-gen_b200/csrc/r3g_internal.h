@@ -106,6 +106,11 @@ inline cudaError_t r3g_launch_pdl(r3g_ctx* ctx, void (*kernel)(KArgs...), dim3 g
 }
 #endif
 
+// Connected components of a triangle mesh (mesh.cu): labels[v] = smallest vertex index of v's component, launched on `s`
+// without a synchronise.  An index outside [0, nv) sets *bad_dev; skip_dead ignores faces whose first index is negative.
+int r3g_launch_components(r3g_ctx* ctx, const int32_t* faces, int64_t nf, int64_t nv, int32_t* labels, int* bad_dev,
+                          bool skip_dead, cudaStream_t s);
+
 // 2D..4D fp16 tensor map with 128B swizzle; dims/strides innermost first, strides in BYTES for dims >= 1.
 int r3g_make_tmap_f16(r3g_ctx* ctx, CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                       const uint64_t* strides_bytes, const uint32_t* box);

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(PKG_DIR))
 CSRC = os.path.join(os.path.dirname(PKG_DIR), "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libr3g.so")
 
-CU_SOURCES = ["ctx.cu", "mc.cu", "mesh.cu", "rowops.cu", "heads.cu", "conv.cu", "gemm.cu", "attn.cu"]
+CU_SOURCES = ["ctx.cu", "mc.cu", "mesh.cu", "decimate.cu", "rowops.cu", "heads.cu", "conv.cu", "gemm.cu", "attn.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
@@ -38,7 +38,7 @@ def _nvcc():
 def build_cuda(force=False, verbose=False):
     srcs = [os.path.join(CSRC, s) for s in CU_SOURCES]
     deps = srcs + [os.path.join(CSRC, h) for h in os.listdir(CSRC) if h.endswith((".h", ".cuh"))]
-    deps += [os.path.join(ROOT, "include", "r3g.h"), os.path.join(ROOT, "include", "r3g_mc_tables.h")]
+    deps += [os.path.join(ROOT, "include", h) for h in ("r3g.h", "r3g_decimate.h", "r3g_mc_tables.h")]
     if not force and _newer(LIB_PATH, deps):
         return LIB_PATH
     objs = []

@@ -25,7 +25,7 @@ def _ptr(t, dev, op, arg):
 # one in an integer slot reaches ctypes unconverted and is refused there, and _launch looks at a few arguments instead
 # of all of them (the wrappers' host cost is on the timed path of the eager conditioner and ShapeVAE)
 _PTR_ARGS = {name[len("r3g_"):]: [i for i, t in enumerate(argtypes[1:-1]) if t is C.c_void_p]
-             for name, (_, argtypes) in _abi.SIGNATURES.items()}
+             for name, (_, argtypes) in {**_abi.SIGNATURES, **_abi.DECIMATE_SIGNATURES}.items()}
 
 
 def _launch(name, anchor, *args):
@@ -513,6 +513,36 @@ def mesh_components(faces, num_vertices):
     labels = torch.empty(int(num_vertices), device=faces.device, dtype=torch.int32)
     _launch("mesh_components", f, f, f.shape[0], int(num_vertices), labels)
     return labels
+
+
+_DECIMATE_WS = {}
+
+
+def mesh_decimate(verts, faces, target):
+    """Quadric edge-collapse decimation to `target` faces (see include/r3g_decimate.h): verts CUDA float32 [V, 3], faces
+    CUDA int32 [F, 3] on the same device.  Returns (verts float32 [V', 3], faces int32 [F', 3], rounds) on that device,
+    F' in {target - 1, target} when the collapse rules allow it, else the smallest mesh they allow.  The workspace is
+    cached per device like the marching-cubes one."""
+    if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
+        raise TypeError("verts must be float32 [V, 3]")
+    if faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise TypeError("faces must be int32 [F, 3]")
+    if int(target) < 0:
+        raise ValueError(f"mesh_decimate: target must be >= 0, got {target}")
+    v, f = verts.contiguous(), faces.contiguous()
+    nv, nf = v.shape[0], f.shape[0]
+    ws_bytes = _abi.load_library().r3g_decimate_workspace_bytes(nv, nf)
+    if ws_bytes == 0 and nv and nf:
+        raise ValueError(f"mesh_decimate: {nv} vertices / {nf} faces exceed the int32 index range")
+    ws = _DECIMATE_WS.get(v.device)
+    if ws is None or ws.numel() < ws_bytes:
+        ws = _DECIMATE_WS[v.device] = torch.empty(max(ws_bytes, 1), device=v.device, dtype=torch.uint8)
+    v_out = torch.empty_like(v)
+    f_out = torch.empty_like(f)
+    nv_out, nf_out, rounds = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+    _launch("mesh_decimate", v, v, nv, f, nf, int(target), ws, ws_bytes, v_out, f_out, C.byref(nv_out), C.byref(nf_out),
+            C.byref(rounds))
+    return v_out[:nv_out.value], f_out[:nf_out.value], rounds.value
 
 
 def mc_classify(grid, level=0.0):

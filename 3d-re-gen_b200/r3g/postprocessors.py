@@ -11,7 +11,12 @@ marching-cubes output stays on the GPU.
                          (postprocessors.py:146-152): mirrored as the identity on (vertices, faces).
   FaceReducer            quadric edge-collapse decimation to 40 000 faces is MeshLab's algorithm; pymeshlab is not
                          installed here, there is neither an output nor a specification to pin against: meshes at or
-                         under the limit pass through, larger ones raise NotImplementedError.
+                         under the limit pass through, larger ones raise NotImplementedError.  FaceReducerR3G is the
+                         face reduction this project runs instead.
+  FaceReducerR3G         r3g's own quadric edge-collapse decimation (r3g_mesh_decimate, include/r3g_decimate.h) with the
+                         reference filter's settings fixed: boundary weight 3, normal, topology and quality guards,
+                         autoclean.  Rounds of independent collapses on the GPU, deterministic; not MeshLab's collapse
+                         order.
 Inputs / outputs: Latent2MeshOutput (numpy or CUDA tensors) or a (vertices, faces) pair; tensors stay on their device."""
 import numpy as np
 import torch
@@ -66,8 +71,31 @@ class DegenerateFaceRemover:
 
 
 class FaceReducer:
+    """MeshLab's decimation, which is not mirrored: meshes over the limit raise.  FaceReducerR3G reduces them."""
+
     def __call__(self, mesh, max_facenum=40000):
         _, f = _unpack(mesh)
         if max_facenum > len(f):
             return mesh
-        raise NotImplementedError("quadric edge-collapse decimation (pymeshlab) is not mirrored; see the module docstring")
+        raise NotImplementedError("quadric edge-collapse decimation (pymeshlab) is not mirrored; see the module docstring "
+                                  "(FaceReducerR3G is r3g's own)")
+
+
+class FaceReducerR3G:
+    """Reduce a mesh to at most max_facenum faces (max_facenum - 1 or max_facenum when the collapse rules allow) on the
+    GPU.  A mesh with fewer faces is returned as it is; numpy in, numpy out; tensors stay on their device."""
+
+    def __call__(self, mesh, max_facenum=40000, device="cuda"):
+        v, f = _unpack(mesh)
+        if max_facenum > len(f):
+            return mesh
+        as_numpy = not torch.is_tensor(v)
+        if as_numpy:
+            vt = torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(device)
+            ft = torch.from_numpy(np.ascontiguousarray(f, dtype=np.int32)).to(device)
+        else:
+            vt, ft = v.to(torch.float32), f.to(device=v.device, dtype=torch.int32)
+        v2, f2, _ = ops.mesh_decimate(vt, ft, int(max_facenum))
+        if as_numpy:
+            v2, f2 = v2.cpu().numpy(), f2.cpu().numpy()
+        return _repack(mesh, v2, f2)

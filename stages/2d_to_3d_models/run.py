@@ -12,9 +12,10 @@ Differences, all on purpose:
     the SORTED list, and the finished meshes are gathered to rank 0 (r3g/dist.py::MeshBatchGatherer, over NCCL
     when there is more than one rank), which writes each .glb as its mesh lands;
   * FloaterRemover runs on the GPU (r3g/postprocessors.py: union-find components, MeshLab's 0.5 % rule) and
-    DegenerateFaceRemover is the reference's no-op round trip; FaceReducer (pymeshlab quadric decimation to 40 000 faces)
-    and the texture pipeline are not mirrored (SURVEY.md section 8f rows 2 and 4) -- the .glb holds the cleaned,
-    undecimated, untextured shape;
+    DegenerateFaceRemover is the reference's no-op round trip; the face reduction to 40 000 faces is FaceReducerR3G,
+    r3g's own quadric edge collapse on the GPU (FaceReducer, pymeshlab's decimation, is not mirrored: same settings,
+    not MeshLab's collapse order); the texture pipeline is not mirrored (SURVEY.md section 8f row 4) -- the .glb holds
+    the cleaned, reduced, untextured shape;
   * `--random-weights` builds the Hunyuan3D-2 architecture with seeded random weights when no checkpoint is
     reachable (this build environment has no network).
 
@@ -37,7 +38,7 @@ sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
 
 from r3g.dist import MeshBatchGatherer, shard_indices  # noqa: E402
 from r3g.pipelines import Hunyuan3DDiTFlowMatchingPipeline, SimpleMesh  # noqa: E402
-from r3g.postprocessors import DegenerateFaceRemover, FloaterRemover  # noqa: E402
+from r3g.postprocessors import DegenerateFaceRemover, FaceReducerR3G, FloaterRemover  # noqa: E402
 
 
 def load_config(path):
@@ -103,11 +104,14 @@ def main():
         v, f = out.mesh_v, out.mesh_f
         if not torch.is_tensor(v):
             v, f = torch.from_numpy(v), torch.from_numpy(f)
-        # src/2d_to_3d_models/run.py:93-94 (FaceReducer, :95, is not mirrored)
+        # src/2d_to_3d_models/run.py:93-95, with FaceReducerR3G for FaceReducer (descent winding, before the flip below)
         v, f = DegenerateFaceRemover()(FloaterRemover()((v, f), device=f"cuda:{local}"))
+        raw_faces = f.shape[0]
+        v, f = FaceReducerR3G()((v, f), device=f"cuda:{local}")
         local_meshes.append((v, f))
         local_names.append(stem)
-        print(f"[rank {rank}] {stem}: {v.shape[0]} vertices, {f.shape[0]} faces in {time.time() - t0:.2f} s", flush=True)
+        print(f"[rank {rank}] {stem}: {v.shape[0]} vertices, {f.shape[0]} faces (reduced from {raw_faces}) in "
+              f"{time.time() - t0:.2f} s", flush=True)
 
     all_names = [local_names]
     if world > 1:
