@@ -1,4 +1,4 @@
-// Quadric edge-collapse decimation on the device (include/r3g_decimate.h describes the algorithm): the face reduction of
+// Quadric edge-collapse decimation on the device (include/r3g.h describes the algorithm): the face reduction of
 // stage 3 (src/2d_to_3d_models/run.py:95).  Each round rebuilds the adjacency from the face array (half-edges sorted by
 // vertex pair, a vertex -> face CSR), prices every edge, selects an independent set by two rounds of 64-bit atomicMin
 // and applies it in place.  Every float64 operation is an explicit _rn intrinsic, so the numpy mirror
@@ -7,7 +7,6 @@
 #include <cub/cub.cuh>
 
 #include "r3g_internal.h"
-#include "../../include/r3g_decimate.h"
 
 namespace {
 
@@ -401,58 +400,59 @@ __global__ void out_faces_kernel(const int* __restrict__ faces, const int* __res
 }
 
 // ---- workspace ----------------------------------------------------------------------------------------------------
-struct Layout {
-  size_t pos, Q, remap, label, comp_nv, comp_sel, comp_min, vflag, m, M, vf_cnt, vf_off, vf_cur, vref, vnew;
-  size_t faces, vf_list, hkey_in, hkey, hval_in, hval, head, eidx, estart, he_edge, ekey, ep, esel, skey, skey_sorted;
-  size_t fkeep, fnew, cnt, total;
+struct Workspace {
+  // per vertex
+  double *pos, *Q;      // position (3), quadric (10)
+  int *remap, *label, *comp_nv, *comp_sel, *vflag, *vf_cnt, *vf_off, *vf_cur, *vref, *vnew;
+  u64 *comp_min, *m, *M;
+  // per half-edge (3 per face)
+  int *faces, *vf_list, *hval_in, *hval, *head, *eidx, *estart, *he_edge, *esel;
+  u64 *hkey_in, *hkey, *ekey, *skey, *skey_sorted;
+  double* ep;
+  // per face, and the C_* counters
+  int *fkeep, *fnew, *cnt;
 };
 
 bool sizes_ok(int64_t nv, int64_t nf) { return nv >= 0 && nf >= 0 && nv <= 0x7ffffffeLL && 3 * nf <= 0x7ffffffeLL; }
 
-Layout layout(int64_t nv, int64_t nf) {
-  Layout L;
-  size_t o = 0;
-  auto take = [&](size_t bytes) {
-    const size_t at = o;
-    o += (bytes + 255) & ~(size_t)255;
-    return at;
-  };
+// points w's buffers into `base` (null: only measures) and returns the bytes they take
+size_t carve(Workspace& w, char* base, int64_t nv, int64_t nf) {
   const size_t V = (size_t)nv, F = (size_t)nf, H = 3 * F;
-  L.pos = take(V * 3 * 8);
-  L.Q = take(V * 10 * 8);
-  L.remap = take(V * 4);
-  L.label = take(V * 4);
-  L.comp_nv = take(V * 4);
-  L.comp_sel = take(V * 4);
-  L.comp_min = take(V * 8);
-  L.vflag = take(V * 4);
-  L.m = take(V * 8);
-  L.M = take(V * 8);
-  L.vf_cnt = take((V + 1) * 4);
-  L.vf_off = take((V + 1) * 4);
-  L.vf_cur = take(V * 4);
-  L.vref = take((V + 1) * 4);
-  L.vnew = take((V + 1) * 4);
-  L.faces = take(H * 4);
-  L.vf_list = take(H * 4);
-  L.hkey_in = take(H * 8);
-  L.hkey = take(H * 8);
-  L.hval_in = take(H * 4);
-  L.hval = take(H * 4);
-  L.head = take((H + 1) * 4);
-  L.eidx = take((H + 1) * 4);
-  L.estart = take((H + 1) * 4);
-  L.he_edge = take(H * 4);
-  L.ekey = take(H * 8);
-  L.ep = take(H * 3 * 8);
-  L.esel = take(H * 4);
-  L.skey = take(H * 8);
-  L.skey_sorted = take(H * 8);
-  L.fkeep = take((F + 1) * 4);
-  L.fnew = take((F + 1) * 4);
-  L.cnt = take(C_COUNT * 4);
-  L.total = o;
-  return L;
+  r3g_carver c{base};
+  w.pos = c.take<double>(V * 3);
+  w.Q = c.take<double>(V * 10);
+  w.remap = c.take<int>(V);
+  w.label = c.take<int>(V);
+  w.comp_nv = c.take<int>(V);
+  w.comp_sel = c.take<int>(V);
+  w.comp_min = c.take<u64>(V);
+  w.vflag = c.take<int>(V);
+  w.m = c.take<u64>(V);
+  w.M = c.take<u64>(V);
+  w.vf_cnt = c.take<int>(V + 1);
+  w.vf_off = c.take<int>(V + 1);
+  w.vf_cur = c.take<int>(V);
+  w.vref = c.take<int>(V + 1);
+  w.vnew = c.take<int>(V + 1);
+  w.faces = c.take<int>(H);
+  w.vf_list = c.take<int>(H);
+  w.hkey_in = c.take<u64>(H);
+  w.hkey = c.take<u64>(H);
+  w.hval_in = c.take<int>(H);
+  w.hval = c.take<int>(H);
+  w.head = c.take<int>(H + 1);
+  w.eidx = c.take<int>(H + 1);
+  w.estart = c.take<int>(H + 1);
+  w.he_edge = c.take<int>(H);
+  w.ekey = c.take<u64>(H);
+  w.ep = c.take<double>(H * 3);
+  w.esel = c.take<int>(H);
+  w.skey = c.take<u64>(H);
+  w.skey_sorted = c.take<u64>(H);
+  w.fkeep = c.take<int>(F + 1);
+  w.fnew = c.take<int>(F + 1);
+  w.cnt = c.take<int>(C_COUNT);
+  return c.off;
 }
 
 inline unsigned blocks(int64_t n) { return (unsigned)((n + 255) / 256); }
@@ -470,7 +470,8 @@ struct CubTemp {
 }  // namespace
 
 extern "C" size_t r3g_decimate_workspace_bytes(int64_t nv, int64_t nf) {
-  return sizes_ok(nv, nf) ? layout(nv, nf).total : 0;
+  Workspace w;
+  return sizes_ok(nv, nf) ? carve(w, nullptr, nv, nf) : 0;
 }
 
 extern "C" int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, const int32_t* faces, int64_t nf,
@@ -482,99 +483,67 @@ extern "C" int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, c
       (nf > 0 && (!faces || !faces_out)))
     return r3g_fail(ctx, R3G_E_INVALID, "mesh_decimate: bad arguments (nv %lld, nf %lld, target %lld)", (long long)nv,
                     (long long)nf, (long long)target);
-  const Layout L = layout(nv, nf);
-  if (!workspace || workspace_bytes < L.total)
-    return r3g_fail(ctx, R3G_E_WORKSPACE, "mesh_decimate: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
+  Workspace w;
+  const size_t need = carve(w, (char*)workspace, nv, nf);
+  if (!workspace || workspace_bytes < need)
+    return r3g_fail(ctx, R3G_E_WORKSPACE, "mesh_decimate: workspace of %zu bytes, %zu needed", workspace_bytes, need);
   *nv_out_host = *nf_out_host = 0;
   if (rounds_host) *rounds_host = 0;
   if (nv == 0 || nf == 0) return R3G_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  char* w = (char*)workspace;
-  double* pos = (double*)(w + L.pos);
-  double* Q = (double*)(w + L.Q);
-  int* remap = (int*)(w + L.remap);
-  int* label = (int*)(w + L.label);
-  int* comp_nv = (int*)(w + L.comp_nv);
-  int* comp_sel = (int*)(w + L.comp_sel);
-  u64* comp_min = (u64*)(w + L.comp_min);
-  int* vflag = (int*)(w + L.vflag);
-  u64* m = (u64*)(w + L.m);
-  u64* M = (u64*)(w + L.M);
-  int* vf_cnt = (int*)(w + L.vf_cnt);
-  int* vf_off = (int*)(w + L.vf_off);
-  int* vf_cur = (int*)(w + L.vf_cur);
-  int* vref = (int*)(w + L.vref);
-  int* vnew = (int*)(w + L.vnew);
-  int* wf = (int*)(w + L.faces);
-  int* vf_list = (int*)(w + L.vf_list);
-  u64* hkey_in = (u64*)(w + L.hkey_in);
-  u64* hkey = (u64*)(w + L.hkey);
-  int* hval_in = (int*)(w + L.hval_in);
-  int* hval = (int*)(w + L.hval);
-  int* head = (int*)(w + L.head);
-  int* eidx = (int*)(w + L.eidx);
-  int* estart = (int*)(w + L.estart);
-  int* he_edge = (int*)(w + L.he_edge);
-  u64* ekey = (u64*)(w + L.ekey);
-  double* ep = (double*)(w + L.ep);
-  int* esel = (int*)(w + L.esel);
-  u64* skey = (u64*)(w + L.skey);
-  u64* skey_sorted = (u64*)(w + L.skey_sorted);
-  int* fkeep = (int*)(w + L.fkeep);
-  int* fnew = (int*)(w + L.fnew);
-  int* cnt = (int*)(w + L.cnt);
   int* host = reinterpret_cast<int*>(ctx->pinned);
   const int NV = (int)nv, NF = (int)nf, NH = 3 * NF;
-  const int* n_edges = eidx + NH;
+  const int* n_edges = w.eidx + NH;
 
   CubTemp tmp;
   tmp.s = s;
   {
     size_t b = 0;
-    R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(nullptr, b, hkey_in, hkey, hval_in, hval, NH, 0, 64, s));
+    R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(nullptr, b, w.hkey_in, w.hkey, w.hval_in, w.hval, NH, 0, 64, s));
     tmp.bytes = b;
-    R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortKeys(nullptr, b, skey, skey_sorted, NH, 0, 64, s));
+    R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortKeys(nullptr, b, w.skey, w.skey_sorted, NH, 0, 64, s));
     tmp.bytes = b > tmp.bytes ? b : tmp.bytes;
-    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, head, eidx, NH + 1, s));
+    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, w.head, w.eidx, NH + 1, s));
     tmp.bytes = b > tmp.bytes ? b : tmp.bytes;
-    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, vf_cnt, vf_off, NV + 1, s));
+    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, w.vf_cnt, w.vf_off, NV + 1, s));
     tmp.bytes = b > tmp.bytes ? b : tmp.bytes;
-    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, fkeep, fnew, NF + 1, s));
+    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, w.fkeep, w.fnew, NF + 1, s));
     tmp.bytes = b > tmp.bytes ? b : tmp.bytes;
     R3G_CUDA_OK(ctx, cudaMallocAsync(&tmp.p, tmp.bytes, s));
   }
 
-  R3G_CUDA_OK(ctx, cudaMemsetAsync(cnt, 0, C_COUNT * sizeof(int), s));
-  init_faces_kernel<<<blocks(NF), 256, 0, s>>>(faces, nf, nv, wf, cnt);
+  R3G_CUDA_OK(ctx, cudaMemsetAsync(w.cnt, 0, C_COUNT * sizeof(int), s));
+  init_faces_kernel<<<blocks(NF), 256, 0, s>>>(faces, nf, nv, w.faces, w.cnt);
   R3G_LAUNCH_OK(ctx);
-  init_verts_kernel<<<blocks(NV), 256, 0, s>>>(verts, nv, pos, remap);
+  init_verts_kernel<<<blocks(NV), 256, 0, s>>>(verts, nv, w.pos, w.remap);
   R3G_LAUNCH_OK(ctx);
-  R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, cnt, C_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s));
+  R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, w.cnt, C_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s));
   R3G_CUDA_OK(ctx, cudaStreamSynchronize(s));
   if (host[C_BAD]) return r3g_fail(ctx, R3G_E_INVALID, "mesh_decimate: a face index is outside [0, nv)");
   int64_t live = host[C_NLIVE];
 
   // the adjacency of the current face array: sorted half-edges, edges, boundary / frozen flags, vertex -> face CSR
   auto adjacency = [&]() -> int {
-    halfedge_kernel<<<blocks(NH), 256, 0, s>>>(wf, NH, hkey_in, hval_in);
+    halfedge_kernel<<<blocks(NH), 256, 0, s>>>(w.faces, NH, w.hkey_in, w.hval_in);
     R3G_LAUNCH_OK(ctx);
-    R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, hkey_in, hkey, hval_in, hval, NH, 0, 64, s));
-    head_kernel<<<blocks(NH + 1), 256, 0, s>>>(hkey, NH, head);
+    R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, w.hkey_in, w.hkey, w.hval_in, w.hval, NH, 0, 64,
+                                                     s));
+    head_kernel<<<blocks(NH + 1), 256, 0, s>>>(w.hkey, NH, w.head);
     R3G_LAUNCH_OK(ctx);
-    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, head, eidx, NH + 1, s));
-    edge_kernel<<<blocks(NH), 256, 0, s>>>(hkey, hval, head, eidx, NH, estart, he_edge);
+    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, w.head, w.eidx, NH + 1, s));
+    edge_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.hval, w.head, w.eidx, NH, w.estart, w.he_edge);
     R3G_LAUNCH_OK(ctx);
-    R3G_CUDA_OK(ctx, cudaMemsetAsync(vflag, 0, nv * sizeof(int), s));
-    vertex_flag_kernel<<<blocks(NH), 256, 0, s>>>(hkey, estart, n_edges, NH, vflag);
+    R3G_CUDA_OK(ctx, cudaMemsetAsync(w.vflag, 0, nv * sizeof(int), s));
+    vertex_flag_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.estart, n_edges, NH, w.vflag);
     R3G_LAUNCH_OK(ctx);
-    R3G_CUDA_OK(ctx, cudaMemsetAsync(vf_cnt, 0, (nv + 1) * sizeof(int), s));
-    R3G_CUDA_OK(ctx, cudaMemsetAsync(vf_cur, 0, nv * sizeof(int), s));
-    vf_count_kernel<<<blocks(NF), 256, 0, s>>>(wf, NF, vf_cnt);
+    R3G_CUDA_OK(ctx, cudaMemsetAsync(w.vf_cnt, 0, (nv + 1) * sizeof(int), s));
+    R3G_CUDA_OK(ctx, cudaMemsetAsync(w.vf_cur, 0, nv * sizeof(int), s));
+    vf_count_kernel<<<blocks(NF), 256, 0, s>>>(w.faces, NF, w.vf_cnt);
     R3G_LAUNCH_OK(ctx);
-    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, vf_cnt, vf_off, NV + 1, s));
-    vf_fill_kernel<<<blocks(NF), 256, 0, s>>>(wf, NF, vf_off, vf_cur, vf_list);
+    R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, w.vf_cnt, w.vf_off, NV + 1, s));
+    vf_fill_kernel<<<blocks(NF), 256, 0, s>>>(w.faces, NF, w.vf_off, w.vf_cur, w.vf_list);
     R3G_LAUNCH_OK(ctx);
-    vf_sort_kernel<<<blocks(NV), 256, 0, s>>>(vf_off, NV, vf_list);
+    vf_sort_kernel<<<blocks(NV), 256, 0, s>>>(w.vf_off, NV, w.vf_list);
     R3G_LAUNCH_OK(ctx);
     return R3G_OK;
   };
@@ -582,46 +551,47 @@ extern "C" int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, c
   int64_t rounds = 0;
   if (live > target) {
     if (int rc = adjacency()) return rc;
-    quadric_kernel<<<blocks(NV), 256, 0, s>>>(wf, pos, vf_off, vf_list, estart, he_edge, NV, Q);
+    quadric_kernel<<<blocks(NV), 256, 0, s>>>(w.faces, w.pos, w.vf_off, w.vf_list, w.estart, w.he_edge, NV, w.Q);
     R3G_LAUNCH_OK(ctx);
-    if (int rc = r3g_launch_components(ctx, wf, nf, nv, label, cnt + C_BAD, true, s)) return rc;
-    R3G_CUDA_OK(ctx, cudaMemsetAsync(comp_nv, 0, nv * sizeof(int), s));
-    component_size_kernel<<<blocks(NV), 256, 0, s>>>(vf_off, label, NV, comp_nv);
+    if (int rc = r3g_launch_components(ctx, w.faces, nf, nv, w.label, w.cnt + C_BAD, true, s)) return rc;
+    R3G_CUDA_OK(ctx, cudaMemsetAsync(w.comp_nv, 0, nv * sizeof(int), s));
+    component_size_kernel<<<blocks(NV), 256, 0, s>>>(w.vf_off, w.label, NV, w.comp_nv);
     R3G_LAUNCH_OK(ctx);
     while (live > target) {
       if (rounds > 0)
         if (int rc = adjacency()) return rc;
-      R3G_CUDA_OK(ctx, cudaMemsetAsync(m, 0xff, nv * sizeof(u64), s));
-      cost_kernel<<<blocks(NH), 256, 0, s>>>(hkey, estart, n_edges, NH, wf, vf_off, vf_list, vflag, label, comp_nv, pos,
-                                             Q, ekey, ep, m);
+      R3G_CUDA_OK(ctx, cudaMemsetAsync(w.m, 0xff, nv * sizeof(u64), s));
+      cost_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.estart, n_edges, NH, w.faces, w.vf_off, w.vf_list, w.vflag,
+                                             w.label, w.comp_nv, w.pos, w.Q, w.ekey, w.ep, w.m);
       R3G_LAUNCH_OK(ctx);
-      R3G_CUDA_OK(ctx, cudaMemcpyAsync(M, m, nv * sizeof(u64), cudaMemcpyDeviceToDevice, s));
-      ring_kernel<<<blocks(NH), 256, 0, s>>>(hkey, estart, n_edges, NH, m, M);
+      R3G_CUDA_OK(ctx, cudaMemcpyAsync(w.M, w.m, nv * sizeof(u64), cudaMemcpyDeviceToDevice, s));
+      ring_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.estart, n_edges, NH, w.m, w.M);
       R3G_LAUNCH_OK(ctx);
-      R3G_CUDA_OK(ctx, cudaMemsetAsync(comp_sel, 0, nv * sizeof(int), s));
-      R3G_CUDA_OK(ctx, cudaMemsetAsync(comp_min, 0xff, nv * sizeof(u64), s));
-      select_kernel<<<blocks(NH), 256, 0, s>>>(hkey, estart, n_edges, NH, ekey, M, label, esel, comp_sel, comp_min);
+      R3G_CUDA_OK(ctx, cudaMemsetAsync(w.comp_sel, 0, nv * sizeof(int), s));
+      R3G_CUDA_OK(ctx, cudaMemsetAsync(w.comp_min, 0xff, nv * sizeof(u64), s));
+      select_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.estart, n_edges, NH, w.ekey, w.M, w.label, w.esel, w.comp_sel,
+                                               w.comp_min);
       R3G_LAUNCH_OK(ctx);
-      R3G_CUDA_OK(ctx, cudaMemsetAsync(cnt + C_NSEL, 0, 2 * sizeof(int), s));
-      component_trim_kernel<<<blocks(NH), 256, 0, s>>>(hkey, estart, n_edges, NH, ekey, label, comp_nv, comp_sel,
-                                                       comp_min, esel, skey, cnt);
+      R3G_CUDA_OK(ctx, cudaMemsetAsync(w.cnt + C_NSEL, 0, 2 * sizeof(int), s));
+      component_trim_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.estart, n_edges, NH, w.ekey, w.label, w.comp_nv,
+                                                       w.comp_sel, w.comp_min, w.esel, w.skey, w.cnt);
       R3G_LAUNCH_OK(ctx);
-      R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, cnt, C_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s));
+      R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, w.cnt, C_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s));
       R3G_CUDA_OK(ctx, cudaStreamSynchronize(s));
       const int nsel = host[C_NSEL];
       if (nsel == 0) break;
       const int64_t k = (live - target + 1) / 2;
       if (nsel > k) {      // the last round: only the k cheapest, so the count lands on target or target - 1
-        R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortKeys(tmp.p, tmp.bytes, skey, skey_sorted, NH, 0, 64, s));
-        cut_kernel<<<blocks(NH), 256, 0, s>>>(n_edges, NH, ekey, skey_sorted, (int)k, esel);
+        R3G_CUDA_OK(ctx, cub::DeviceRadixSort::SortKeys(tmp.p, tmp.bytes, w.skey, w.skey_sorted, NH, 0, 64, s));
+        cut_kernel<<<blocks(NH), 256, 0, s>>>(n_edges, NH, w.ekey, w.skey_sorted, (int)k, w.esel);
         R3G_LAUNCH_OK(ctx);
       }
-      apply_kernel<<<blocks(NH), 256, 0, s>>>(hkey, hval, estart, n_edges, NH, esel, ep, label, pos, Q, remap, wf,
-                                              comp_nv, cnt);
+      apply_kernel<<<blocks(NH), 256, 0, s>>>(w.hkey, w.hval, w.estart, n_edges, NH, w.esel, w.ep, w.label, w.pos, w.Q,
+                                              w.remap, w.faces, w.comp_nv, w.cnt);
       R3G_LAUNCH_OK(ctx);
-      rewrite_kernel<<<blocks(NF), 256, 0, s>>>(wf, NF, remap);
+      rewrite_kernel<<<blocks(NF), 256, 0, s>>>(w.faces, NF, w.remap);
       R3G_LAUNCH_OK(ctx);
-      R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, cnt, C_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s));
+      R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, w.cnt, C_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s));
       R3G_CUDA_OK(ctx, cudaStreamSynchronize(s));
       live -= host[C_REMOVED];
       ++rounds;
@@ -629,17 +599,17 @@ extern "C" int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, c
   }
 
   // stable compaction of the surviving faces and the vertices they reference
-  R3G_CUDA_OK(ctx, cudaMemsetAsync(vref, 0, (nv + 1) * sizeof(int), s));
-  mark_kernel<<<blocks(NF + 1), 256, 0, s>>>(wf, NF, vref, fkeep);
+  R3G_CUDA_OK(ctx, cudaMemsetAsync(w.vref, 0, (nv + 1) * sizeof(int), s));
+  mark_kernel<<<blocks(NF + 1), 256, 0, s>>>(w.faces, NF, w.vref, w.fkeep);
   R3G_LAUNCH_OK(ctx);
-  R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, vref, vnew, NV + 1, s));
-  R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, fkeep, fnew, NF + 1, s));
-  out_verts_kernel<<<blocks(NV), 256, 0, s>>>(pos, vref, vnew, NV, verts_out);
+  R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, w.vref, w.vnew, NV + 1, s));
+  R3G_CUDA_OK(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, w.fkeep, w.fnew, NF + 1, s));
+  out_verts_kernel<<<blocks(NV), 256, 0, s>>>(w.pos, w.vref, w.vnew, NV, verts_out);
   R3G_LAUNCH_OK(ctx);
-  out_faces_kernel<<<blocks(NF), 256, 0, s>>>(wf, fkeep, fnew, vnew, NF, faces_out);
+  out_faces_kernel<<<blocks(NF), 256, 0, s>>>(w.faces, w.fkeep, w.fnew, w.vnew, NF, faces_out);
   R3G_LAUNCH_OK(ctx);
-  R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, vnew + nv, sizeof(int), cudaMemcpyDeviceToHost, s));
-  R3G_CUDA_OK(ctx, cudaMemcpyAsync(host + 1, fnew + nf, sizeof(int), cudaMemcpyDeviceToHost, s));
+  R3G_CUDA_OK(ctx, cudaMemcpyAsync(host, w.vnew + nv, sizeof(int), cudaMemcpyDeviceToHost, s));
+  R3G_CUDA_OK(ctx, cudaMemcpyAsync(host + 1, w.fnew + nf, sizeof(int), cudaMemcpyDeviceToHost, s));
   R3G_CUDA_OK(ctx, cudaStreamSynchronize(s));
   *nv_out_host = host[0];
   *nf_out_host = host[1];

@@ -632,42 +632,35 @@ int make_dims(r3g_ctx* ctx, int n0, int n1, int n2, McDims& d) {
   return R3G_OK;
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 constexpr int kBitsGridMax = 148 * 8 * 2;     // upper bound used for the workspace (the launch uses num_sms * 8)
 
-size_t carve_sizes(int n0, int n1, int n2, McWorkspace* w, char* base) {
+// points w's buffers into `base` (null: only measures) and returns the bytes they take
+size_t carve_sizes(int n0, int n1, int n2, McWorkspace& w, char* base) {
   const int64_t npts = (int64_t)n0 * n1 * n2;
   const int64_t ncells = (int64_t)(n0 - 1) * (n1 - 1) * (n2 - 1);
   const int64_t nwords = (npts / 128) * 4 + 6;      // whole 128-point groups + the tail's words + padding
   const int64_t nsegs = (int64_t)(n0 - 1) * (n1 - 1) * ((n2 - 1 + 31) / 32);
   const size_t seg_blocks = (size_t)((nsegs + kThreads - 1) / kThreads);
   const size_t cell_blocks = (size_t)((ncells + kThreads - 1) / kThreads);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += align256(bytes); return p; };
-  char* vid = take(sizeof(int32_t) * 4 * (size_t)npts);
-  char* bits = take(sizeof(unsigned) * (size_t)nwords);
-  char* act = take(sizeof(unsigned) * (size_t)nsegs);
-  char* list = take(sizeof(unsigned) * (size_t)ncells);
-  char* info = take(sizeof(unsigned short) * (size_t)ncells);
-  char* seg_sum = take(sizeof(unsigned) * seg_blocks);
-  char* seg_off = take(sizeof(unsigned) * seg_blocks);
-  char* cell_counts = take(sizeof(uint2) * cell_blocks);
-  char* cell_off = take(sizeof(uint2) * cell_blocks);
-  char* minmax = take(sizeof(unsigned) * 2 * kBitsGridMax);
-  char* totals = take(256);
-  if (w) {
-    w->vid = (int32_t*)vid; w->bits = (unsigned*)bits; w->act = (unsigned*)act; w->list = (unsigned*)list;
-    w->info = (unsigned short*)info; w->seg_sum = (unsigned*)seg_sum; w->seg_off = (unsigned*)seg_off;
-    w->cell_counts = (uint2*)cell_counts; w->cell_off = (uint2*)cell_off; w->minmax = (unsigned*)minmax;
-    w->totals = (int64_t*)totals;
-    w->seg_blocks = (int)seg_blocks; w->cell_blocks_max = (int)cell_blocks;
-  }
-  return off;
+  r3g_carver c{base};
+  w.vid = c.take<int32_t>(4 * (size_t)npts);
+  w.bits = c.take<unsigned>((size_t)nwords);
+  w.act = c.take<unsigned>((size_t)nsegs);
+  w.list = c.take<unsigned>((size_t)ncells);
+  w.info = c.take<unsigned short>((size_t)ncells);
+  w.seg_sum = c.take<unsigned>(seg_blocks);
+  w.seg_off = c.take<unsigned>(seg_blocks);
+  w.cell_counts = c.take<uint2>(cell_blocks);
+  w.cell_off = c.take<uint2>(cell_blocks);
+  w.minmax = c.take<unsigned>(2 * kBitsGridMax);
+  w.totals = c.take<int64_t>(5);
+  w.seg_blocks = (int)seg_blocks;
+  w.cell_blocks_max = (int)cell_blocks;
+  return c.off;
 }
 
 int carve(r3g_ctx* ctx, const McDims& d, void* ws, size_t ws_bytes, McWorkspace& w) {
-  const size_t need = carve_sizes(d.n0, d.n1, d.n2, &w, (char*)ws);
+  const size_t need = carve_sizes(d.n0, d.n1, d.n2, w, (char*)ws);
   if (need > ws_bytes || !ws) return r3g_fail(ctx, R3G_E_WORKSPACE, "mc: workspace %zu < required %zu", ws_bytes, need);
   const int groups_per_block = kWarps * 4;
   const int64_t want = (d.npts / 128 + groups_per_block - 1) / groups_per_block + 1;
@@ -683,7 +676,8 @@ int list_grid(const r3g_ctx* ctx, int per_sm) { return ctx->num_sms * per_sm; }
 
 extern "C" size_t r3g_mc_workspace_bytes(int n0, int n1, int n2) {
   if (n0 < 2 || n1 < 2 || n2 < 2) return 0;
-  return carve_sizes(n0, n1, n2, nullptr, nullptr);
+  McWorkspace w;
+  return carve_sizes(n0, n1, n2, w, nullptr);
 }
 
 extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, void* workspace,

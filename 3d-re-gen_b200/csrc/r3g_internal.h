@@ -64,6 +64,19 @@ static inline int r3g_fail(r3g_ctx* ctx, int code, const char* fmt, ...) {
 // host-side test of the 16-byte alignment that 128-bit accesses and tensor-map bases need (a null pointer passes)
 static inline bool r3g_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// Layout of a caller-supplied workspace: buffers in the order they are taken, each rounded up to 256 bytes.  A null
+// base only measures: every take returns nullptr, and `off` ends as the bytes the workspace needs either way.
+struct r3g_carver {
+  char* base;
+  size_t off = 0;
+  template <typename T>
+  T* take(size_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += (count * sizeof(T) + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
 #define R3G_CUDA_OK(ctx, expr)                                                                         \
   do {                                                                                                 \
     cudaError_t _e = (expr);                                                                           \

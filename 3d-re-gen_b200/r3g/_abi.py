@@ -1,4 +1,4 @@
-"""ctypes binding of include/r3g.h and include/r3g_decimate.h.  This is the only place that touches the C ABI.
+"""ctypes binding of include/r3g.h.  This is the only place that touches the C ABI.
 
 There is NO fallback: if libr3g.so is missing or no CUDA device is present, the first compute call
 raises.  (`load_library()` itself works without a GPU so that the CPU test-suite can check the
@@ -63,6 +63,9 @@ SIGNATURES = {
     "r3g_mc_extract": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp, _sz, _vp, _vp, _vp]),
     "r3g_mc_classify": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp]),
     "r3g_mesh_components": (_i, [_vp, _vp, _i64, _i64, _vp, _vp]),
+    "r3g_decimate_workspace_bytes": (_sz, [_i64, _i64]),
+    "r3g_mesh_decimate": (_i, [_vp, _vp, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, C.POINTER(_i64), C.POINTER(_i64),
+                               C.POINTER(_i64), _vp]),
     "r3g_linear": (_i, [_vp, C.POINTER(LinearArgs), _vp]),
     "r3g_attention": (_i, [_vp, C.POINTER(AttentionArgs), _vp]),
     "r3g_layernorm": (_i, [_vp, _vp, _i64, _vp, _i64, _i, _i, _f, _vp, _vp, _vp, _vp, _i64, _i, _i, _i64, _i64, _vp]),
@@ -86,13 +89,6 @@ SIGNATURES = {
     "r3g_unproject": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
 }
 
-# the same for include/r3g_decimate.h, compiled into the same library
-DECIMATE_SIGNATURES = {
-    "r3g_decimate_workspace_bytes": (_sz, [_i64, _i64]),
-    "r3g_mesh_decimate": (_i, [_vp, _vp, _i64, _vp, _i64, _i64, _vp, _sz, _vp, _vp, C.POINTER(_i64), C.POINTER(_i64),
-                               C.POINTER(_i64), _vp]),
-}
-
 _lib = None
 _lock = threading.Lock()
 
@@ -114,7 +110,7 @@ def load_library():
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'`. "
                 "r3g has no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
-        for name, (res, args) in {**SIGNATURES, **DECIMATE_SIGNATURES}.items():
+        for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)
             fn.restype = res
             fn.argtypes = args

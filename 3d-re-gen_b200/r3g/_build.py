@@ -38,7 +38,7 @@ def _nvcc():
 def build_cuda(force=False, verbose=False):
     srcs = [os.path.join(CSRC, s) for s in CU_SOURCES]
     deps = srcs + [os.path.join(CSRC, h) for h in os.listdir(CSRC) if h.endswith((".h", ".cuh"))]
-    deps += [os.path.join(ROOT, "include", h) for h in ("r3g.h", "r3g_decimate.h", "r3g_mc_tables.h")]
+    deps += [os.path.join(ROOT, "include", h) for h in ("r3g.h", "r3g_mc_tables.h")]
     if not force and _newer(LIB_PATH, deps):
         return LIB_PATH
     objs = []

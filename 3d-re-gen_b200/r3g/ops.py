@@ -25,7 +25,7 @@ def _ptr(t, dev, op, arg):
 # one in an integer slot reaches ctypes unconverted and is refused there, and _launch looks at a few arguments instead
 # of all of them (the wrappers' host cost is on the timed path of the eager conditioner and ShapeVAE)
 _PTR_ARGS = {name[len("r3g_"):]: [i for i, t in enumerate(argtypes[1:-1]) if t is C.c_void_p]
-             for name, (_, argtypes) in {**_abi.SIGNATURES, **_abi.DECIMATE_SIGNATURES}.items()}
+             for name, (_, argtypes) in _abi.SIGNATURES.items()}
 
 
 def _launch(name, anchor, *args):
@@ -459,16 +459,17 @@ class MarchingCubesError(RuntimeError):
     pass
 
 
-_MC_WS = {}
+_WS = {}
 
 
-def _mc_workspace(device, nbytes):
-    """One cached marching-cubes workspace per device (0.39 GB at 257^3, 3.0 GB at 513^3; sized for the worst case of every
-    cell crossed): not re-requested from the allocator per object."""
-    ws = _MC_WS.get(device)
+def _workspace(kind, device, nbytes):
+    """One cached byte workspace per kind ("mc", "decimate") and device, grown when a call needs more and never shrunk:
+    not re-requested from the allocator per object (marching cubes: 0.39 GB at 257^3, 3.0 GB at 513^3, sized for the
+    worst case of every cell crossed).  The kinds stay apart: the marching-cubes one carries r3g_mc_count's state to
+    r3g_mc_extract."""
+    ws = _WS.get((kind, device))
     if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(nbytes, device=device, dtype=torch.uint8)
-        _MC_WS[device] = ws
+        ws = _WS[kind, device] = torch.empty(max(nbytes, 1), device=device, dtype=torch.uint8)
     return ws
 
 
@@ -480,7 +481,7 @@ def marching_cubes(grid, level=0.0, bounds=None):
     grid = grid.contiguous()
     n0, n1, n2 = grid.shape
     ws_bytes = _abi.load_library().r3g_mc_workspace_bytes(n0, n1, n2)
-    ws = _mc_workspace(grid.device, ws_bytes)
+    ws = _workspace("mc", grid.device, ws_bytes)
     nv, nf = C.c_int64(0), C.c_int64(0)
     try:
         _launch("mc_count", grid, grid, n0, n1, n2, float(level), ws, ws_bytes, C.byref(nv), C.byref(nf))
@@ -515,11 +516,8 @@ def mesh_components(faces, num_vertices):
     return labels
 
 
-_DECIMATE_WS = {}
-
-
 def mesh_decimate(verts, faces, target):
-    """Quadric edge-collapse decimation to `target` faces (see include/r3g_decimate.h): verts CUDA float32 [V, 3], faces
+    """Quadric edge-collapse decimation to `target` faces (see include/r3g.h): verts CUDA float32 [V, 3], faces
     CUDA int32 [F, 3] on the same device.  Returns (verts float32 [V', 3], faces int32 [F', 3], rounds) on that device,
     F' in {target - 1, target} when the collapse rules allow it, else the smallest mesh they allow.  The workspace is
     cached per device like the marching-cubes one."""
@@ -534,9 +532,7 @@ def mesh_decimate(verts, faces, target):
     ws_bytes = _abi.load_library().r3g_decimate_workspace_bytes(nv, nf)
     if ws_bytes == 0 and nv and nf:
         raise ValueError(f"mesh_decimate: {nv} vertices / {nf} faces exceed the int32 index range")
-    ws = _DECIMATE_WS.get(v.device)
-    if ws is None or ws.numel() < ws_bytes:
-        ws = _DECIMATE_WS[v.device] = torch.empty(max(ws_bytes, 1), device=v.device, dtype=torch.uint8)
+    ws = _workspace("decimate", v.device, ws_bytes)
     v_out = torch.empty_like(v)
     f_out = torch.empty_like(f)
     nv_out, nf_out, rounds = C.c_int64(0), C.c_int64(0), C.c_int64(0)

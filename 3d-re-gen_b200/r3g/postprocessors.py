@@ -13,7 +13,7 @@ marching-cubes output stays on the GPU.
                          installed here, there is neither an output nor a specification to pin against: meshes at or
                          under the limit pass through, larger ones raise NotImplementedError.  FaceReducerR3G is the
                          face reduction this project runs instead.
-  FaceReducerR3G         r3g's own quadric edge-collapse decimation (r3g_mesh_decimate, include/r3g_decimate.h) with the
+  FaceReducerR3G         r3g's own quadric edge-collapse decimation (r3g_mesh_decimate, include/r3g.h) with the
                          reference filter's settings fixed: boundary weight 3, normal, topology and quality guards,
                          autoclean.  Rounds of independent collapses on the GPU, deterministic; not MeshLab's collapse
                          order.
@@ -41,14 +41,24 @@ def _repack(mesh, v, f):
     return v, f
 
 
+def _to_tensors(v, f, device, v_dtype=None):
+    """numpy arrays or tensors -> vertices (cast to v_dtype if one is given) and int32 faces as tensors on `device`."""
+    if not torch.is_tensor(v):
+        v, f = torch.from_numpy(np.ascontiguousarray(v)), torch.from_numpy(np.ascontiguousarray(f))
+    return v.to(device=device, dtype=v_dtype), f.to(device=device, dtype=torch.int32)
+
+
+def _like_input(v_in, v, f):
+    """The result (v, f) as numpy arrays if the input's vertices v_in were not a tensor."""
+    return (v, f) if torch.is_tensor(v_in) else (v.cpu().numpy(), f.cpu().numpy())
+
+
 class FloaterRemover:
     nbfaceratio = 0.005
 
     def __call__(self, mesh, device="cuda"):
         v, f = _unpack(mesh)
-        as_numpy = not torch.is_tensor(v)
-        vt = torch.as_tensor(np.ascontiguousarray(v) if as_numpy else v).to(device)
-        ft = torch.as_tensor(np.ascontiguousarray(f) if as_numpy else f).to(device=device, dtype=torch.int32)
+        vt, ft = _to_tensors(v, f, device)
         if ft.shape[0] == 0:
             return mesh
         labels = ops.mesh_components(ft, vt.shape[0]).long()
@@ -60,9 +70,7 @@ class FloaterRemover:
         new_index = torch.cumsum(keep_vert, 0, dtype=torch.int64) - 1
         v2 = vt[keep_vert]
         f2 = new_index[ft[keep_face].long()].to(torch.int32)
-        if as_numpy:
-            v2, f2 = v2.cpu().numpy(), f2.cpu().numpy()
-        return _repack(mesh, v2, f2)
+        return _repack(mesh, *_like_input(v, v2, f2))
 
 
 class DegenerateFaceRemover:
@@ -89,13 +97,7 @@ class FaceReducerR3G:
         v, f = _unpack(mesh)
         if max_facenum > len(f):
             return mesh
-        as_numpy = not torch.is_tensor(v)
-        if as_numpy:
-            vt = torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(device)
-            ft = torch.from_numpy(np.ascontiguousarray(f, dtype=np.int32)).to(device)
-        else:
-            vt, ft = v.to(torch.float32), f.to(device=v.device, dtype=torch.int32)
+        # `device` is where numpy input goes; tensors stay on the vertices' device
+        vt, ft = _to_tensors(v, f, v.device if torch.is_tensor(v) else device, torch.float32)
         v2, f2, _ = ops.mesh_decimate(vt, ft, int(max_facenum))
-        if as_numpy:
-            v2, f2 = v2.cpu().numpy(), f2.cpu().numpy()
-        return _repack(mesh, v2, f2)
+        return _repack(mesh, *_like_input(v, v2, f2))

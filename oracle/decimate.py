@@ -1,4 +1,4 @@
-"""ORACLE -- test infrastructure only.  numpy mirror of r3g_mesh_decimate (include/r3g_decimate.h describes the algorithm,
+"""ORACLE -- test infrastructure only.  numpy mirror of r3g_mesh_decimate (include/r3g.h describes the algorithm,
 3d-re-gen_b200/csrc/decimate.cu implements it): the same rounds, vectorised per round, with the same float64 operations in
 the same order -- elementwise only, no matmul / einsum / axis reductions whose summation order numpy may choose -- so the
 two agree bit for bit.  Importable from tests/ and tools/."""

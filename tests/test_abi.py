@@ -56,10 +56,10 @@ def test_every_compute_call_refuses_a_context_without_device(lib):
     here), names itself in the error, and launches nothing."""
     from r3g import _abi
     not_compute = {"r3g_version", "r3g_create", "r3g_destroy", "r3g_last_error", "r3g_launch_count",
-                   "r3g_mc_workspace_bytes"}
+                   "r3g_mc_workspace_bytes", "r3g_decimate_workspace_bytes"}
     calls = [(name, [t() for t in argtypes[1:]]) for name, (_, argtypes) in sorted(_abi.SIGNATURES.items())
              if name not in not_compute]
-    assert len(calls) == 25
+    assert len(calls) == 26
     handle = ctypes.c_void_p()
     assert lib.r3g_create(-1, ctypes.byref(handle)) == _abi.R3G_E_CUDA and handle
     try:
@@ -84,6 +84,16 @@ def test_marching_cubes_workspace_size(lib):
         assert b <= 1.05 * (16 * n ** 3 + n ** 3 // 8 + 6 * (n - 1) ** 3) + (1 << 20)      # + masks, scan arrays, alignment
         prev = b
     assert lib.r3g_mc_workspace_bytes(7, 12, 9) > 0
+
+
+def test_decimate_workspace_size(lib):
+    """Pure arithmetic: grows with both sizes, 256-byte granular, 0 where the int32 limits are exceeded."""
+    b = lib.r3g_decimate_workspace_bytes
+    assert b(100, 200) > 0 and b(100, 200) % 256 == 0
+    assert b(1000, 200) > b(100, 200) and b(100, 2000) > b(100, 200)
+    n = 1 << 20
+    assert 150 * n <= b(n, 0) - b(0, 0) <= 200 * n and 280 * n <= b(0, n) - b(0, 0) <= 330 * n
+    assert b(1 << 31, 10) == 0 and b(10, 1 << 30) == 0 and b(-1, 10) == 0
 
 
 def test_product_package_does_not_import_oracle():

@@ -69,6 +69,7 @@ VALID = [
     _unproject,
     lambda ops: ops.marching_cubes(f(5, 5, 5), 0.0, bounds=[-1.0] * 3 + [1.0] * 3),
     lambda ops: ops.mesh_components(torch.zeros(4, 3, dtype=torch.int32), 6),
+    lambda ops: ops.mesh_decimate(f(6, 3), torch.zeros(4, 3, dtype=torch.int32), 2),
     lambda ops: ops.mc_classify(f(5, 5, 5)),
 ]
 
@@ -118,8 +119,9 @@ def test_argument_lists_match_the_c_signatures(ops, calls):
     for call, good, _ in OUTS.values():
         call(ops, good)
     compute = {name for name in _abi.SIGNATURES if name not in {
-        "r3g_version", "r3g_create", "r3g_destroy", "r3g_last_error", "r3g_launch_count", "r3g_mc_workspace_bytes"}}
-    assert len(compute) == 25
+        "r3g_version", "r3g_create", "r3g_destroy", "r3g_last_error", "r3g_launch_count", "r3g_mc_workspace_bytes",
+        "r3g_decimate_workspace_bytes"}}
+    assert len(compute) == 26
     assert {name for name, _ in calls} == compute
     for name, args in calls:
         argtypes = _abi.SIGNATURES[name][1]
@@ -129,6 +131,7 @@ def test_argument_lists_match_the_c_signatures(ops, calls):
                 argtype.from_param(arg)
             except TypeError as e:
                 pytest.fail(f"{name} argument {i} = {arg!r} does not convert to {argtype.__name__}: {e}")
+    assert ops._PTR_ARGS["mesh_decimate"] == [0, 2, 5, 7, 8]
 
 
 def test_tensor_arguments_must_live_on_the_launch_device(ops):
