@@ -351,8 +351,8 @@ constexpr int kGemvRows = 4;   // output rows per warp, their weight loads issue
 template <int BT>
 __global__ void __launch_bounds__(256) gemv_kernel(const __half* __restrict__ w, const __half* __restrict__ bias,
                                                    const __half* __restrict__ vec, int64_t vec_ld,
-                                                   __half* __restrict__ out, int64_t out_ld, int B, int N, int K,
-                                                   int silu_in, int silu_out) {
+                                                   __half* out, int64_t out_ld, const __half* residual, int B, int N,
+                                                   int K, int silu_in, int silu_out) {
   extern __shared__ float gemv_x[];   // [BT][K]
   pdl_wait();      // vec is the previous kernel's output
   pdl_trigger();
@@ -412,6 +412,8 @@ __global__ void __launch_bounds__(256) gemv_kernel(const __half* __restrict__ w,
           v = rnd_h(v);
           v = v / (1.f + expf(-v));
         }
+        // residual may alias out: this lane reads the element before it writes it
+        if (residual) v = rnd_h(v) + h2f(residual[(int64_t)b * out_ld + n]);
         out[(int64_t)b * out_ld + n] = __float2half_rn(v);
       }
     }
@@ -434,21 +436,26 @@ __global__ void timestep_embedding_kernel(const __half* __restrict__ t, __half* 
 }
 
 // ------------------------------------------------------------------------------------------- CFG + Euler
+// nb = 2: v = cat(cond, uncond), mixed with the guidance scale first.  nb = 1: v is the prediction itself (a model run
+// without CFG), guidance is not read.
 __global__ void cfg_euler_kernel(__half* __restrict__ x, const __half* __restrict__ v, __half* __restrict__ x_dup,
-                                 int64_t n, float guidance, float dsigma) {
+                                 int64_t n, int nb, float guidance, float dsigma) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float vc = h2f(v[i]), vu = h2f(v[n + i]);
-  // noise_pred_uncond + g * (cond - uncond), each op rounded to fp16 (pipelines.py:753)
-  const float mix = rnd_h(vu + rnd_h(guidance * rnd_h(vc - vu)));
+  float mix = h2f(v[i]);
+  if (nb == 2) {
+    const float vc = mix, vu = h2f(v[n + i]);
+    // noise_pred_uncond + g * (cond - uncond), each op rounded to fp16 (pipelines.py:753)
+    mix = rnd_h(vu + rnd_h(guidance * rnd_h(vc - vu)));
+  }
   // (sigma_next - sigma) is a 0-dim fp32 tensor: the product takes the fp16 dtype of model_output,
-  // the sum is fp32 (schedulers.py:300-309)
+  // the sum is fp32 (schedulers.py:300-309, :462-469)
   const float step = rnd_h(dsigma * mix);
   const __half r = __float2half_rn(h2f(x[i]) + step);
   x[i] = r;
   if (x_dup) {
     x_dup[i] = r;
-    x_dup[n + i] = r;
+    if (nb == 2) x_dup[n + i] = r;
   }
 }
 
@@ -778,7 +785,8 @@ extern "C" int r3g_qk_norm(r3g_ctx* ctx, void* buf, int64_t ld, int rows, int he
 }
 
 extern "C" int r3g_gemv(r3g_ctx* ctx, const void* w, const void* bias, const void* vec, int64_t vec_ld, void* out,
-                        int64_t out_ld, int B, int N, int K, int silu_in, int silu_out, void* stream) {
+                        int64_t out_ld, const void* residual, int B, int N, int K, int silu_in, int silu_out,
+                        void* stream) {
   R3G_ENTRY(ctx, "gemv");
   if (B < 1 || B > kGemvMaxB || K % 8 || vec_ld % 8)
     return r3g_fail(ctx, R3G_E_INVALID, "gemv: B in [1,%d], K %% 8 == 0 required", kGemvMaxB);
@@ -789,7 +797,8 @@ extern "C" int r3g_gemv(r3g_ctx* ctx, const void* w, const void* bias, const voi
   const unsigned grid = (unsigned)((N + 8 * kGemvRows - 1) / (8 * kGemvRows));
   auto args = [&](auto kern) {
     return r3g_launch_pdl(ctx, kern, dim3(grid), dim3(256), smem, (cudaStream_t)stream, (const __half*)w,
-                          (const __half*)bias, (const __half*)vec, vec_ld, (__half*)out, out_ld, B, N, K, silu_in, silu_out);
+                          (const __half*)bias, (const __half*)vec, vec_ld, (__half*)out, out_ld, (const __half*)residual, B, N, K, silu_in,
+                          silu_out);
   };
   R3G_CUDA_OK(ctx, bt == 1 ? args(gemv_kernel<1>) : bt == 2 ? args(gemv_kernel<2>) : bt == 4 ? args(gemv_kernel<4>)
                                                                                               : args(gemv_kernel<8>));
@@ -807,11 +816,12 @@ extern "C" int r3g_timestep_embedding(r3g_ctx* ctx, const void* t_f16, void* out
   return R3G_OK;
 }
 
-extern "C" int r3g_cfg_euler_step(r3g_ctx* ctx, void* x, const void* v, void* x_dup, int64_t n, float guidance,
-                                  float dsigma, void* stream) {
+extern "C" int r3g_cfg_euler_step(r3g_ctx* ctx, void* x, const void* v, void* x_dup, int64_t n, int nb,
+                                  float guidance, float dsigma, void* stream) {
   R3G_ENTRY(ctx, "cfg_euler_step");
+  if (nb != 1 && nb != 2) return r3g_fail(ctx, R3G_E_INVALID, "cfg_euler_step: nb must be 1 or 2, got %d", nb);
   cfg_euler_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>((__half*)x, (const __half*)v,
-                                                                                    (__half*)x_dup, n, guidance,
+                                                                                    (__half*)x_dup, n, nb, guidance,
                                                                                     dsigma);
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;

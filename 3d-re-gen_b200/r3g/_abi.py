@@ -73,10 +73,10 @@ SIGNATURES = {
     "r3g_qk_norm_rope": (_i, [_vp, _vp, _i64, _i64, _i, _f, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _vp]),
     "r3g_patchify": (_i, [_vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp, _vp, _vp]),
     "r3g_qk_norm": (_i, [_vp, _vp, _i64, _i, _i, _i64, _i64, _i64, _i, _f, _vp, _vp, _vp, _vp, _i, _i64, _vp]),
-    "r3g_gemv": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _i, _vp]),
+    "r3g_gemv": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _i, _i, _i, _i, _i, _vp]),
     "r3g_swiglu": (_i, [_vp, _vp, _i64, _vp, _i64, _i64, _i, _vp]),
     "r3g_timestep_embedding": (_i, [_vp, _vp, _vp, _i, _i, _f, _f, _vp]),
-    "r3g_cfg_euler_step": (_i, [_vp, _vp, _vp, _vp, _i64, _f, _f, _vp]),
+    "r3g_cfg_euler_step": (_i, [_vp, _vp, _vp, _vp, _i64, _i, _f, _f, _vp]),
     "r3g_grid_fourier": (_i, [_vp, _vp, _i64, _i64, _i64, _i, _vp, _i, _i, _vp]),
     "r3g_points_fourier": (_i, [_vp, _vp, _vp, _i64, _i64, _i, _i, _vp]),
     "r3g_points_fourier_f32": (_i, [_vp, _vp, _vp, _i64, _i64, _i, _i, _vp]),

@@ -26,8 +26,6 @@ class Hunyuan3DDiT:
             raise ValueError(f"Hidden size {hidden_size} must be divisible by num_heads {num_heads}")
         if hidden_size // num_heads != 64:
             raise ValueError("r3g attention kernels are built for head_dim 64 (Hunyuan3D-2's geometry)")
-        if guidance_embed:
-            raise NotImplementedError("guidance-distilled checkpoints are not on the 3D-RE-GEN path")
         if dtype != torch.float16:
             raise ValueError("the reference runs this model in float16 (pipelines.py:205); so does r3g")
         self.in_channels = in_channels
@@ -41,7 +39,8 @@ class Hunyuan3DDiT:
         self.depth_single_blocks = depth_single_blocks
         self.qkv_bias = qkv_bias
         self.time_factor = time_factor
-        self.guidance_embed = False
+        # guidance-distilled (-fast / -turbo) checkpoints: the guidance scale is a model input (guidance_in)
+        self.guidance_embed = bool(guidance_embed)
         self.device = torch.device(device)
         self.dtype = dtype
         self.w = None
@@ -72,7 +71,10 @@ class Hunyuan3DDiT:
             return t.detach().to(device=dev, dtype=torch.float16).contiguous()
 
         w = {}
-        for n in ("latent_in", "time_in.in_layer", "time_in.out_layer", "cond_in", "final_layer.linear"):
+        names = ["latent_in", "time_in.in_layer", "time_in.out_layer", "cond_in", "final_layer.linear"]
+        if self.guidance_embed:
+            names += ["guidance_in.in_layer", "guidance_in.out_layer"]
+        for n in names:
             w[n + ".weight"], w[n + ".bias"] = g(n + ".weight"), g(n + ".bias")
         mod_w, mod_b, self.mod_off = [], [], {}
         off = 0
@@ -125,6 +127,9 @@ class Hunyuan3DDiT:
         lin(sd, "latent_in", H, self.in_channels, 0.05)
         lin(sd, "time_in.in_layer", H, 256)
         lin(sd, "time_in.out_layer", H, H)
+        if self.guidance_embed:
+            lin(sd, "guidance_in.in_layer", H, 256)
+            lin(sd, "guidance_in.out_layer", H, H)
         lin(sd, "cond_in", H, self.context_in_dim)
         for i in range(self.depth):
             p = f"double_blocks.{i}."
@@ -162,6 +167,8 @@ class Hunyuan3DDiT:
             e = lambda *s: torch.empty(*s, device=dev, dtype=torch.float16)  # noqa: E731
             ws = dict(X=e(B, L, H), XM=e(B, L, H), QKV=e(B, L, 3 * H), HID=e(B, L, Mh), S1=e(B, L, 3 * H + Mh),
                       mods=e(B, self.mod_total), temb=e(B, 256), vec0=e(B, H), vec=e(B, H), out=e(B, Li, self.out_channels))
+            if self.guidance_embed:
+                ws.update(gemb=e(B, 256), gvec0=e(B, H))
             self._ws[key] = ws
         return ws
 
@@ -171,8 +178,11 @@ class Hunyuan3DDiT:
         m = ws["mods"]
         return [m[:, off + i * H: off + (i + 1) * H] for i in range(n)]
 
-    def forward(self, x, t, contexts, uncond_txt_shared=False, **kwargs):
+    def forward(self, x, t, contexts, uncond_txt_shared=False, guidance=None, **kwargs):
         """x: [B, Li, in_channels] fp16, t: [B] fp16 in [0,1], contexts['main']: [B, Lt, context_in_dim] fp16.
+
+        guidance: [B] fp16, the guidance scale of each sample; required by (and only read by) a guidance-distilled model
+        (guidance_embed), which adds guidance_in(timestep_embedding(guidance)) to the time embedding.
 
         uncond_txt_shared: B == 2 (cond, uncond) and every text row of contexts['main'][1] is the same vector.  t is the
         same for both samples too, so those Lt rows stay equal through every block (all ops but attention are
@@ -190,6 +200,8 @@ class Hunyuan3DDiT:
         H, Mh, nh = self.hidden_size, self.mlp_hidden, self.num_heads
         if uncond_txt_shared and B != 2:
             raise ValueError(f"uncond_txt_shared needs the (cond, uncond) batch of 2, got B = {B}")
+        if self.guidance_embed and guidance is None:
+            raise ValueError("Didn't get guidance strength for guidance distilled model.")   # hunyuan3ddit.py:394-395
         ws = self._workspace(B, Li, Lt)
         X, XM, QKV, HID, S1 = ws["X"], ws["XM"], ws["QKV"], ws["HID"], ws["S1"]
         txt, img = X[:, :Lt], X[:, Lt:]
@@ -198,6 +210,14 @@ class Hunyuan3DDiT:
         ops.timestep_embedding(t, 256, 1000.0, float(self.time_factor), out=ws["temb"])
         ops.gemv(w["time_in.in_layer.weight"], w["time_in.in_layer.bias"], ws["temb"], silu_out=True, out=ws["vec0"])
         ops.gemv(w["time_in.out_layer.weight"], w["time_in.out_layer.bias"], ws["vec0"], out=ws["vec"])
+        if self.guidance_embed:
+            # vec = vec + guidance_in(timestep_embedding(guidance, 256, self.time_factor)) (hunyuan3ddit.py:396): the
+            # same positional max_period = 1000, and guidance * 1000 is evaluated in fp16 like t * 1000
+            ops.timestep_embedding(guidance, 256, 1000.0, float(self.time_factor), out=ws["gemb"])
+            ops.gemv(w["guidance_in.in_layer.weight"], w["guidance_in.in_layer.bias"], ws["gemb"], silu_out=True,
+                     out=ws["gvec0"])
+            ops.gemv(w["guidance_in.out_layer.weight"], w["guidance_in.out_layer.bias"], ws["gvec0"],
+                     residual=ws["vec"], out=ws["vec"])
         ops.gemv(w["mod.weight"], w["mod.bias"], ws["vec"], silu_in=True, out=ws["mods"])
         ops.linear(x, w["latent_in.weight"], w["latent_in.bias"], out=img)
         ops.linear(cond, w["cond_in.weight"], w["cond_in.bias"], out=txt)

@@ -287,13 +287,19 @@ def qk_norm_(buf, heads, q_off, k_off, head_stride, mode, eps, q_w, q_b=None, k_
     return buf
 
 
-def gemv(w, bias, vec, silu_in=False, silu_out=False, out=None):
-    """out[b] = W . act(vec[b]) + bias for B <= 8 rows."""
+def gemv(w, bias, vec, silu_in=False, silu_out=False, out=None, residual=None):
+    """out[b] = W . act(vec[b]) + bias for B <= 8 rows; with residual ([B, N] fp16, it may be out itself)
+    out[b] = fp16(that) + residual[b], rounded again."""
     _f16(w, "w"); _f16(vec, "vec")
     B, K = vec.shape
     N = w.shape[0]
     out = _out("gemv", out, (B, N), torch.float16, vec)
-    _launch("gemv", vec, w, bias, vec, vec.stride(0), out, out.stride(0), B, N, K, int(silu_in), int(silu_out))
+    if residual is not None and (residual.dtype != torch.float16 or residual.shape != out.shape
+                                 or residual.stride() != out.stride()):
+        raise ValueError(f"gemv: residual must be float16 {tuple(out.shape)} with out's strides {out.stride()}, got "
+                         f"{residual.dtype} {tuple(residual.shape)} strides {residual.stride()}")
+    _launch("gemv", vec, w, bias, vec, vec.stride(0), out, out.stride(0), residual, B, N, K, int(silu_in),
+            int(silu_out))
     return out
 
 
@@ -317,15 +323,19 @@ def timestep_embedding(t, dim=256, time_factor=1000.0, max_period=10000.0, out=N
 
 
 def cfg_euler_step_(x, v, guidance, dsigma, x_dup=None):
-    """x <- x + dsigma * (v_uncond + g (v_cond - v_uncond)); v = cat(cond, uncond)."""
+    """x <- x + dsigma * (v_uncond + g (v_cond - v_uncond)) with v = cat(cond, uncond) (v twice x's size), or
+    x <- x + dsigma * v with guidance ignored when v is x's size (a model run without CFG).  x_dup, when given,
+    receives x as many times as v holds samples: the next step's model input."""
     _f16(x, "x"); _f16(v, "v")
     n = x.numel()
-    if v.numel() != 2 * n or not (x.is_contiguous() and v.is_contiguous()):
-        raise ValueError("v must hold cond and uncond predictions, contiguous")
-    if x_dup is not None and (x_dup.dtype != torch.float16 or x_dup.numel() != 2 * n or not x_dup.is_contiguous()):
-        raise ValueError(f"cfg_euler_step_: x_dup must be contiguous float16 with 2 * {n} elements, got {x_dup.dtype} "
+    nb = v.numel() // n if n else 0
+    if v.numel() != nb * n or nb not in (1, 2) or not (x.is_contiguous() and v.is_contiguous()):
+        raise ValueError(f"cfg_euler_step_: v must be contiguous with {n} (no CFG) or 2 * {n} (cond, uncond) elements, "
+                         f"got {tuple(v.shape)}")
+    if x_dup is not None and (x_dup.dtype != torch.float16 or x_dup.numel() != nb * n or not x_dup.is_contiguous()):
+        raise ValueError(f"cfg_euler_step_: x_dup must be contiguous float16 with {nb} * {n} elements, got {x_dup.dtype} "
                          f"{tuple(x_dup.shape)} with strides {x_dup.stride()}")
-    _launch("cfg_euler_step", x, x, v, x_dup, n, float(guidance), float(dsigma))
+    _launch("cfg_euler_step", x, x, v, x_dup, n, nb, float(guidance), float(dsigma))
     return x
 
 

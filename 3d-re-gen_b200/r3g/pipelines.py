@@ -7,7 +7,9 @@ i.e. what src/2d_to_3d_models/run.py:77-84 calls:
                     generator=torch.manual_seed(seed), output_type="trimesh")[0]
 
 Everything between the conditioner output and the mesh runs in libr3g.so: 50 x (CFG-batched DiT forward +
-fused CFG/Euler step), ShapeVAE transformer, dense SDF decode, marching cubes.
+fused CFG/Euler step), ShapeVAE transformer, dense SDF decode, marching cubes.  A guidance-distilled checkpoint
+(`hunyuan3d-dit-v2-0-fast` / `-turbo`: `guidance_embed: true`) runs without CFG, one sample per step with the guidance
+scale as a model input; the `-turbo` config's ConsistencyFlowMatchEulerDiscreteScheduler gives its 5-step schedule.
 """
 import json
 import os
@@ -21,7 +23,7 @@ from .conditioner import DinoImageEncoder, SingleImageEncoder
 from .dit import Hunyuan3DDiT
 from .graphs import GraphCache
 from .preprocessors import ImageProcessorV2
-from .scheduler import FlowMatchEulerDiscreteScheduler, FlowMatchEulerDiscreteSchedulerOutput
+from .scheduler import ConsistencyFlowMatchEulerDiscreteScheduler, FlowMatchEulerDiscreteScheduler
 from .vae import ShapeVAE, SurfaceExtractors
 
 # Hunyuan3D-2 `hunyuan3d-dit-v2-0/config.yaml` values.  The checkpoint config is downloaded at run time by the
@@ -35,6 +37,32 @@ HUNYUAN3D_2_CONFIG = dict(
     scheduler=dict(num_train_timesteps=1000),
     image_processor=dict(size=512, border_ratio=0.15),
 )
+
+# The guidance- and step-distilled `hunyuan3d-dit-v2-0-turbo`: the same architecture plus guidance_in, stepped by
+# ConsistencyFlowMatchEulerDiscreteScheduler.  pcm_timesteps = 100 is UNVERIFIED: the checkpoint's config.yaml is
+# downloaded at run time and is not in the reference tree (the class default is 50).
+HUNYUAN3D_2_TURBO_CONFIG = dict(
+    HUNYUAN3D_2_CONFIG,
+    model=dict(HUNYUAN3D_2_CONFIG["model"], guidance_embed=True),
+    scheduler=dict(target="hy3dgen.shapegen.schedulers.ConsistencyFlowMatchEulerDiscreteScheduler",
+                   num_train_timesteps=1000, pcm_timesteps=100),
+)
+
+
+def _guidance_distilled(model):
+    """pipelines.py:708-711 / :733-735: `hasattr(model, 'guidance_embed') and model.guidance_embed is True`."""
+    return getattr(model, "guidance_embed", False) is True
+
+
+def scheduler_class(target):
+    """The scheduler a config's `scheduler.target` names (pipelines.py:184 instantiates it).  None: the flow-matching
+    scheduler of the base checkpoints."""
+    if target is None or str(target).endswith(".FlowMatchEulerDiscreteScheduler"):
+        return FlowMatchEulerDiscreteScheduler
+    if str(target).endswith(".ConsistencyFlowMatchEulerDiscreteScheduler"):
+        return ConsistencyFlowMatchEulerDiscreteScheduler
+    raise NotImplementedError(f"scheduler target {target!r}: only FlowMatchEulerDiscreteScheduler and "
+                              "ConsistencyFlowMatchEulerDiscreteScheduler (the Hunyuan3D-2 shape checkpoints') are mirrored")
 
 
 class SimpleMesh:
@@ -135,7 +163,8 @@ class Hunyuan3DDiTPipeline:
         cfg = config or HUNYUAN3D_2_CONFIG
         model = Hunyuan3DDiT(device=device, **cfg["model"]).init_random(seed)
         vae = ShapeVAE(device=device, **cfg["vae"]).init_random(seed + 1)
-        sched = FlowMatchEulerDiscreteScheduler(**cfg["scheduler"])
+        sc = dict(cfg["scheduler"])
+        sched = scheduler_class(sc.pop("target", None))(**sc)
         cond = None
         if conditioner == "dinov2":
             torch.manual_seed(seed + 2)
@@ -151,6 +180,7 @@ class Hunyuan3DDiTPipeline:
         import yaml
         with open(config_path) as fh:
             config = yaml.safe_load(fh)
+        sched_cls = scheduler_class(config["scheduler"].get("target"))
         if use_safetensors:
             ckpt_path = ckpt_path.replace(".ckpt", ".safetensors")
         if not os.path.exists(ckpt_path):
@@ -187,7 +217,7 @@ class Hunyuan3DDiTPipeline:
                 raise RuntimeError(f"unexpected conditioner keys (not under {pre!r}): {bad[:5]}")
             enc.model.load_state_dict({k[len(pre):]: v for k, v in ckpt["conditioner"].items()}, strict=True)
             enc.invalidate()
-        return cls(vae=vae, model=model, scheduler=FlowMatchEulerDiscreteScheduler(**config["scheduler"]["params"]),
+        return cls(vae=vae, model=model, scheduler=sched_cls(**config["scheduler"]["params"]),
                    conditioner=SingleImageEncoder(enc),
                    image_processor=ImageProcessorV2(**config["image_processor"]["params"]), device=device,
                    dtype=dtype, **kwargs)
@@ -284,11 +314,12 @@ class Hunyuan3DDiTPipeline:
 class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
 
     def _denoise(self, latents, cond, timesteps, guidance_scale, callback=None, callback_steps=None):
-        """pipelines.py:741-759.  Per step: DiT forward on cat([x, x]) with cat([cond, uncond]) (one CUDA graph
-        replay), then the fused CFG mix + Euler update which also rewrites the duplicated model input."""
+        """pipelines.py:741-759.  Per step: one CUDA graph replay of the DiT forward, then the fused Euler update, which
+        also rewrites the model input.  With CFG the forward runs on cat([x, x]) with cat([cond, uncond]) and the update
+        mixes the two predictions first; without (a guidance-distilled model, or guidance_scale < 0) it runs on x."""
         B = latents.shape[0]
         n = len(timesteps)
-        sig = self.scheduler.sigmas
+        sig = self.scheduler.step_sigmas()
         # timestep = t.expand(B).to(fp16) / num_train_timesteps, evaluated in fp16 as the reference does
         t16 = (timesteps.to(torch.float16) / self.scheduler.config.num_train_timesteps).to(self.device)
         # torch multiplies the fp16 model output by the 0-dim fp32 (sigma_next - sigma) after casting it to the
@@ -296,9 +327,14 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         dsig = [float((sig[i + 1] - sig[i]).to(torch.float16)) for i in range(n)]
         x = latents.contiguous()
         do_cfg = cond["main"].shape[0] == 2 * B
-        x_in = torch.cat([x] * 2) if do_cfg else x
+        x_in = torch.cat([x] * 2) if do_cfg else x.clone()
         t_buf = torch.full((x_in.shape[0],), 0.5, device=self.device, dtype=torch.float16)  # warm-up t; set per step
         ctx = {"main": cond["main"].contiguous()}
+        # pipelines.py:733-737: a guidance-distilled model takes the scale as an input, [guidance_scale] * B in fp16
+        guidance = None
+        if _guidance_distilled(self.model):
+            guidance = torch.tensor([guidance_scale] * x_in.shape[0], dtype=torch.float16).to(self.device)
+        gkw = lambda gs: {} if gs is None else {"guidance": gs}  # noqa: E731  (a model without guidance_in takes none)
         # An unconditional context whose rows are all one vector (the zeros of unconditional_embedding) lets the DiT run
         # that sample on one text row (Hunyuan3DDiT.forward: uncond_txt_shared).  Checked once per call: one sync.
         shared = False
@@ -307,10 +343,15 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
             shared = bool(torch.equal(un, un[:1].expand_as(un)))
         g = None
         if self.use_cuda_graph and self.model.taps is None:
-            g = self._graphs.get((x_in.shape, ctx["main"].shape, shared), (x_in, t_buf, ctx["main"]),
-                                 lambda xs, ts, cs: self.model(xs, ts, {"main": cs}, uncond_txt_shared=shared))
+            g = self._graphs.get((x_in.shape, ctx["main"].shape, shared),
+                                 (x_in, t_buf, ctx["main"]) + ((guidance,) if guidance is not None else ()),
+                                 lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs}, uncond_txt_shared=shared,
+                                                                        **gkw(gs)))
             g.inputs[0].copy_(x_in)
             g.inputs[2].copy_(ctx["main"])
+            if guidance is not None:
+                g.inputs[3].copy_(guidance)
+                guidance = g.inputs[3]
             x_in, t_buf = g.inputs[:2]
         for i in range(n):
             t_buf.copy_(t16[i].expand(x_in.shape[0]))
@@ -319,16 +360,18 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
                 self.replayed_launches += g.launches
                 v = g.outputs
             else:
-                v = self.model(x_in, t_buf, ctx, uncond_txt_shared=shared)
-            if do_cfg:
-                ops.cfg_euler_step_(x, v, guidance_scale, dsig[i], x_dup=x_in)
-            else:
-                ops.cfg_euler_step_(x, torch.cat([v, v]), 0.0, dsig[i], x_dup=None)
-                x_in.copy_(x)
-            if callback is not None and i % callback_steps == 0:
-                # pipelines.py:757-759: callback(step_idx, t, outputs) with outputs.prev_sample = the new latents
+                v = self.model(x_in, t_buf, ctx, uncond_txt_shared=shared, **gkw(guidance))
+            report = callback is not None and i % callback_steps == 0
+            x_prev = x.clone() if report else None
+            ops.cfg_euler_step_(x, v, guidance_scale, dsig[i], x_dup=x_in)
+            if report:
+                # pipelines.py:757-759: callback(step_idx, t, outputs), outputs = what scheduler.step returns
+                mixed = v
+                if do_cfg:
+                    vc, vu = v.chunk(2)
+                    mixed = vu + guidance_scale * (vc - vu)
                 callback(i // getattr(self.scheduler, "order", 1), timesteps[i],
-                         FlowMatchEulerDiscreteSchedulerOutput(prev_sample=x.clone()))   # x is updated in place
+                         self.scheduler.output(i, x_prev, mixed, x.clone()))   # x is updated in place
         return x
 
     @torch.inference_mode()
@@ -337,11 +380,12 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
                  num_chunks=8000, output_type="trimesh", enable_pbar=True, **kwargs):
         callback = kwargs.pop("callback", None)
         callback_steps = kwargs.pop("callback_steps", None)
-        cond = kwargs.pop("cond", None)  # precomputed {'main': [2B, Lt, C]} skips the image encoder (bench/tests)
+        cond = kwargs.pop("cond", None)  # precomputed {'main': [2B or B, Lt, C]} skips the image encoder (bench/tests)
         latents = kwargs.pop("latents", None)
         self.set_surface_extractor(mc_algo)
         device, dtype = self.device, self.dtype
-        do_cfg = guidance_scale >= 0
+        # pipelines.py:708-711: a guidance-distilled model runs without CFG
+        do_cfg = guidance_scale >= 0 and not _guidance_distilled(self.model)
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
         ev[0].record()
         if cond is None:

@@ -234,9 +234,12 @@ int r3g_qk_norm(r3g_ctx* ctx, void* buf, int64_t ld, int rows, int heads, int64_
                 int64_t head_stride, int mode, float eps, const void* q_w, const void* q_b, const void* k_w,
                 const void* k_b, int seg_len, int64_t seg_stride, void* stream);
 /* out[b, :] = W[N,K] . silu?(vec[b, :]) + bias   (tiny-M GEMV: Modulation.lin hunyuan3ddit.py:146-147,
- * MLPEmbedder hunyuan3ddit.py:79-80, LastLayer.adaLN_modulation :275).  fp16 in/out, fp32 accumulate. */
+ * MLPEmbedder hunyuan3ddit.py:79-80, LastLayer.adaLN_modulation :275).  fp16 in/out, fp32 accumulate.
+ * residual (optional, fp16 [B, N] at out_ld; it may alias out): out = fp16(fp16(W . silu?(vec) + bias [, silu]) +
+ * residual), the `vec = vec + guidance_in(...)` of a guidance-distilled model (hunyuan3ddit.py:392-396) in fp16.
+ * residual == NULL writes the GEMV result alone.  out may alias neither vec nor w. */
 int r3g_gemv(r3g_ctx* ctx, const void* w, const void* bias, const void* vec, int64_t vec_ld, void* out,
-             int64_t out_ld, int B, int N, int K, int silu_in, int silu_out, void* stream);
+             int64_t out_ld, const void* residual, int B, int N, int K, int silu_in, int silu_out, void* stream);
 /* SwiGLU gate of the DINOv2-giant conditioner's MLP (Hunyuan3D-2/hy3dgen/shapegen/models/conditioner.py:125-131 runs
  * transformers' Dinov2Model; its Dinov2SwiGLUFFN computes weights_out(silu(x1) * x2) with x1, x2 = weights_in(h).chunk(2)):
  * out[r, j] = fp16(fp16(silu(x[r, j])) * x[r, F + j]) for j < F; x fp16 [rows, >= 2F] (ldx), out fp16 [rows, >= F] (ldo). */
@@ -245,10 +248,14 @@ int r3g_swiglu(r3g_ctx* ctx, const void* x, int64_t ldx, void* out, int64_t ldo,
 int r3g_timestep_embedding(r3g_ctx* ctx, const void* t_f16, void* out, int B, int dim, float time_factor,
                            float max_period, void* stream);
 /* Classifier-free-guidance mix + flow-matching Euler step (pipelines.py:751-756, schedulers.py:300-309):
- *   v = v_uncond + g*(v_cond - v_uncond)  (fp16 arithmetic like the reference), x <- fp16(fp32(x) + dsigma*v).
- * v holds [2*n] halfs (cond first, pipelines.py:752); x holds n halfs; x_dup (optional) receives x twice
- * (the next step's cat([latents]*2), pipelines.py:744). */
-int r3g_cfg_euler_step(r3g_ctx* ctx, void* x, const void* v, void* x_dup, int64_t n, float guidance,
+ *   v = v_uncond + g*(v_cond - v_uncond)  (fp16 arithmetic like the reference), x <- fp16(fp32(x) + fp16(dsigma*v)).
+ * nb is the number of samples in v.  nb = 2: v holds [2*n] halfs (cond first, pipelines.py:752), mixed as above.
+ * nb = 1: v holds n halfs, the prediction of a model run without CFG (pipelines.py:708-711, a guidance-distilled model
+ * or guidance_scale < 0); guidance is ignored and the step is the plain Euler update of schedulers.py:300-309 /
+ * ConsistencyFlowMatchEulerDiscreteScheduler's schedulers.py:462-469.  x holds n halfs; x_dup (optional) receives x nb
+ * times (the next step's model input, cat([latents]*2) or latents, pipelines.py:742-745).  dsigma is the caller's
+ * fp16-rounded sigma_next - sigma.  x, v and x_dup must not overlap. */
+int r3g_cfg_euler_step(r3g_ctx* ctx, void* x, const void* v, void* x_dup, int64_t n, int nb, float guidance,
                        float dsigma, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
