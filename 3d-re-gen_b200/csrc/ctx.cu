@@ -4,7 +4,7 @@
 
 #include "r3g_internal.h"
 
-extern "C" int r3g_version(void) { return 100; }
+extern "C" int r3g_version(void) { return 101; }
 
 extern "C" int r3g_create(int device, r3g_ctx** out) {
   if (!out) return R3G_E_INVALID;

@@ -13,6 +13,9 @@
 // 32-cell mask of a segment with a handful of logic operations, mc_compact writes the crossed cells out in traversal
 // order, and the Lewiner tests, the scans and the two emit passes run one thread per CROSSED cell (dense warps; the
 // eight corner values of those cells are re-read through L2).
+// R3G_MC_DUAL (dual marching cubes, the 'dmc' extractor) shares the passes up to and including the Lewiner decisions and
+// the scans; only its vertex pass (one vertex per connected patch of a cell's tiling) and face pass (one quad per
+// interior sign-changing grid edge) differ, and their output order comes from the same scans.
 #include <float.h>
 
 #include "r3g_internal.h"
@@ -123,23 +126,30 @@ __device__ __forceinline__ int cube_index(const float* raw, float level) {
   return ci;
 }
 
-__device__ __forceinline__ Cell eval_cell(int ci, const float* raw, float level, double* cv, int x, int y, int z) {
-  Cell c;
-  c.ci = ci;
-  c.til = 0; c.nt = 0; c.nv = 0;
-  if (c.ci == 0 || c.ci == 255) return c;
+// The Lewiner tiling of a crossed cell (cube index ci, neither 0 nor 255): face tests, then the interior test where it
+// applies.  Fills cv with the corner values minus the level.  Both extractors take their decisions from here.
+__device__ __forceinline__ int cell_tiling(int ci, const float* raw, float level, double* cv) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) cv[i] = (double)raw[i] - (double)level;
   int sub = 0, j = 0;
-  unsigned amb = r3g_mc_amb_faces[c.ci];
+  unsigned amb = r3g_mc_amb_faces[ci];
   for (int f = 0; f < 6; ++f)
     if (amb & (1u << f)) {
       if (face_pos_connected(cv, f)) sub |= 1 << j;
       ++j;
     }
-  c.til = r3g_mc_tiling_offset[c.ci] + sub;
-  const int idesc = r3g_mc_interior[c.til];
-  if (idesc && interior_joined(cv, idesc)) c.til = r3g_mc_tunnel[c.til];
+  int til = r3g_mc_tiling_offset[ci] + sub;
+  const int idesc = r3g_mc_interior[til];
+  if (idesc && interior_joined(cv, idesc)) til = r3g_mc_tunnel[til];
+  return til;
+}
+
+__device__ __forceinline__ Cell eval_cell(int ci, const float* raw, float level, double* cv, int x, int y, int z) {
+  Cell c;
+  c.ci = ci;
+  c.til = 0; c.nt = 0; c.nv = 0;
+  if (c.ci == 0 || c.ci == 255) return c;
+  c.til = cell_tiling(c.ci, raw, level, cv);
   int t0 = r3g_mc_tiling_start[c.til], t1 = r3g_mc_tiling_start[c.til + 1];
   c.nt = (t1 - t0) / 3;
   unsigned seen = 0;
@@ -448,8 +458,23 @@ __global__ void __launch_bounds__(kThreads) mc_compact_kernel(const unsigned* __
   }
 }
 
+// Dual marching cubes: the grid edges a cell owns, as a mask over the array axes (bit a: the edge along axis a).  A
+// sign-changing grid edge whose four incident cells all lie in the grid gives one quad; its owner is the first of the
+// four in traversal order, the one whose maximum corner (corner 6) the edge touches: local edge 10 (axis 0, corners
+// 2-6), 5 (axis 1, corners 5-6) or 6 (axis 2, corners 7-6).
+__device__ __forceinline__ unsigned dual_owned(int ci, const McDims& d, int x, int y, int z) {
+  const int up = (ci >> 6) & 1;
+  unsigned m = 0;
+  if (x + 1 < d.c2 && y + 1 < d.c1 && up != ((ci >> 2) & 1)) m |= 1u;
+  if (x + 1 < d.c2 && z + 1 < d.c0 && up != ((ci >> 5) & 1)) m |= 2u;
+  if (y + 1 < d.c1 && z + 1 < d.c0 && up != ((ci >> 7) & 1)) m |= 4u;
+  return m;
+}
+
 // Pass 3: the Lewiner tests, one thread per crossed cell: the info word of the cell and, per block of 256 list entries,
-// the (vertex, triangle) counts.
+// the (vertex, triangle) counts.  kDual: the cell's vertices are its patches (r3g_mc_dual_npatch) and its triangles two
+// per owned quad.
+template <bool kDual>
 __global__ void __launch_bounds__(kThreads) mc_eval_kernel(const float* __restrict__ g, McDims d, float level,
                                                            const unsigned* __restrict__ list,
                                                            const int64_t* __restrict__ totals,
@@ -466,9 +491,17 @@ __global__ void __launch_bounds__(kThreads) mc_eval_kernel(const float* __restri
       float raw[8];
       load_cell(g, d, x, y, z, raw);
       double cv[8];
-      const Cell c = eval_cell(cube_index(raw, level), raw, level, cv, x, y, z);
-      info[k] = pack_info(c.til, c.nv);
-      cnt[0] = c.nv; cnt[1] = c.nt;
+      const int ci = cube_index(raw, level);
+      if (kDual) {
+        const int til = cell_tiling(ci, raw, level, cv);      // a listed cell is crossed: ci is neither 0 nor 255
+        const int np = r3g_mc_dual_npatch[til];
+        info[k] = pack_info(til, np);
+        cnt[0] = np; cnt[1] = 2u * __popc(dual_owned(ci, d, x, y, z));
+      } else {
+        const Cell c = eval_cell(ci, raw, level, cv, x, y, z);
+        info[k] = pack_info(c.til, c.nv);
+        cnt[0] = c.nv; cnt[1] = c.nt;
+      }
     }
     unsigned excl[2], tot[2];
     block_scan<2>(cnt, excl, tot);
@@ -593,6 +626,132 @@ __global__ void __launch_bounds__(kThreads) mc_face_kernel(McDims d, const unsig
   }
 }
 
+// Dual marching cubes keeps, per crossed cell, (first vertex id, tiling | cube index << 16) in the first 8 of the 16
+// vertex-id bytes of the cell's origin point: the face pass finds the vertex of a neighbour's patch from it.
+__device__ __forceinline__ int2* dual_cell(int32_t* vid, const McDims& d, int x, int y, int z) {
+  return reinterpret_cast<int2*>(vid + 4 * (((int64_t)z * d.n1 + y) * d.n2 + x));
+}
+
+// crossing of the cell edge a -> b along one array axis: p_a + t (p_b - p_a), corners at integer positions
+__device__ __forceinline__ double dual_cross(int pa, int pb, double t) {
+  return __dadd_rn((double)pa, __dmul_rn(t, __dsub_rn((double)pb, (double)pa)));
+}
+
+// Dual pass 4: every crossed cell writes one vertex per patch, in patch order (patches are numbered by their smallest
+// cube edge): the mean of the patch's edge crossings, t = v_a / (v_a - v_b), summed in increasing edge order, divided by
+// the edge count and by (n_axis - 1), every float64 operation explicitly rounded; stored float32 in array-axis order.
+__global__ void __launch_bounds__(kThreads) mc_dual_vertex_kernel(const float* __restrict__ g, McDims d, float level,
+                                                                  const unsigned* __restrict__ list,
+                                                                  const int64_t* __restrict__ totals,
+                                                                  const unsigned short* __restrict__ info,
+                                                                  const uint2* __restrict__ block_offsets,
+                                                                  int32_t* __restrict__ vid, float* __restrict__ verts) {
+  const int64_t nactive = totals[4];
+  const int64_t nblocks = (nactive + kThreads - 1) / kThreads;
+  for (int64_t kb = blockIdx.x; kb < nblocks; kb += gridDim.x) {
+    const int64_t k = kb * kThreads + threadIdx.x;
+    const unsigned word = k < nactive ? info[k] : 0u;
+    const unsigned np[1] = {word >> 10};
+    unsigned excl[1], tot[1];
+    block_scan<1>(np, excl, tot);
+    if (np[0] == 0) continue;
+    int x, y, z;
+    slot_coords(d, list[k], x, y, z);
+    const int til = word & 1023;
+    float raw[8];
+    load_cell(g, d, x, y, z, raw);
+    double cv[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) cv[i] = (double)raw[i] - (double)level;
+    const unsigned id = block_offsets[kb].x + excl[0];
+    *dual_cell(vid, d, x, y, z) = make_int2((int)id, til | (cube_index(raw, level) << 16));
+    const unsigned char* patch = &r3g_mc_dual_patch[12 * til];
+    for (unsigned p = 0; p < np[0]; ++p) {
+      double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+      int n = 0;
+      for (int e = 0; e < 12; ++e) {
+        if (patch[e] != p) continue;
+        const int a = r3g_mc_edge_corner[2 * e], b = r3g_mc_edge_corner[2 * e + 1];
+        const unsigned char *oa = &r3g_mc_corner_xyz[3 * a], *ob = &r3g_mc_corner_xyz[3 * b];
+        const double t = __ddiv_rn(cv[a], __dsub_rn(cv[a], cv[b]));
+        s0 = __dadd_rn(s0, dual_cross(z + oa[2], z + ob[2], t));
+        s1 = __dadd_rn(s1, dual_cross(y + oa[1], y + ob[1], t));
+        s2 = __dadd_rn(s2, dual_cross(x + oa[0], x + ob[0], t));
+        ++n;
+      }
+      float* out = verts + 3 * (int64_t)(id + p);
+      out[0] = (float)__ddiv_rn(__ddiv_rn(s0, (double)n), (double)d.c0);
+      out[1] = (float)__ddiv_rn(__ddiv_rn(s1, (double)n), (double)d.c1);
+      out[2] = (float)__ddiv_rn(__ddiv_rn(s2, (double)n), (double)d.c2);
+    }
+  }
+}
+
+// The quad of the grid edge an owner cell holds along array axis a: the four cells around the edge as offsets
+// (dx, dy, dz) from the owner, and the cube edge the grid edge is in each of them, counter-clockwise seen from the
+// edge's upper end (q0 = the owner).
+__device__ const unsigned char kDualQuad[3][4][4] = {
+    {{0, 0, 0, 10}, {0, 1, 0, 9}, {1, 1, 0, 8}, {1, 0, 0, 11}},   // axis 0 (z): cells in the (y, x) plane
+    {{0, 0, 0, 5}, {1, 0, 0, 7}, {1, 0, 1, 3}, {0, 0, 1, 1}},     // axis 1 (y): cells in the (x, z) plane
+    {{0, 0, 0, 6}, {0, 0, 1, 2}, {0, 1, 1, 0}, {0, 1, 0, 4}},     // axis 2 (x): cells in the (z, y) plane
+};
+
+__device__ __forceinline__ double dual_dist2(const float* __restrict__ verts, int i, int j) {
+  const float *p = verts + 3 * (int64_t)i, *q = verts + 3 * (int64_t)j;
+  const double d0 = __dsub_rn((double)p[0], (double)q[0]), d1 = __dsub_rn((double)p[1], (double)q[1]);
+  const double d2 = __dsub_rn((double)p[2], (double)q[2]);
+  return __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2));
+}
+
+// Dual pass 5: every crossed cell writes the two triangles of each quad it owns, axes 0, 1, 2 in turn.  The quad is
+// wound so that its normal points towards increasing values (the edge's upper end above the level: counter-clockwise
+// from there) and split along its shorter diagonal (squared float64 lengths of the float32 vertices; a tie takes 0-2).
+__global__ void __launch_bounds__(kThreads) mc_dual_face_kernel(McDims d, const unsigned* __restrict__ list,
+                                                                const int64_t* __restrict__ totals,
+                                                                const uint2* __restrict__ block_offsets,
+                                                                int32_t* __restrict__ vid,
+                                                                const float* __restrict__ verts,
+                                                                int32_t* __restrict__ faces) {
+  const int64_t nactive = totals[4];
+  const int64_t nblocks = (nactive + kThreads - 1) / kThreads;
+  for (int64_t kb = blockIdx.x; kb < nblocks; kb += gridDim.x) {
+    const int64_t k = kb * kThreads + threadIdx.x;
+    int x = 0, y = 0, z = 0;
+    int2 own_cell = make_int2(0, 0);
+    unsigned own = 0;
+    if (k < nactive) {
+      slot_coords(d, list[k], x, y, z);
+      own_cell = *dual_cell(vid, d, x, y, z);
+      own = dual_owned(own_cell.y >> 16, d, x, y, z);
+    }
+    const unsigned nt[1] = {2u * __popc(own)};
+    unsigned excl[1], tot[1];
+    block_scan<1>(nt, excl, tot);
+    if (own == 0) continue;
+    const bool up = (own_cell.y >> 22) & 1;      // corner 6, the upper end of every owned edge, is above the level
+    int64_t fo = 3 * (int64_t)(block_offsets[kb].y + excl[0]);
+    for (int a = 0; a < 3; ++a) {
+      if (!((own >> a) & 1u)) continue;
+      int q[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const unsigned char* c = kDualQuad[a][j];
+        const int2 cell = j == 0 ? own_cell : *dual_cell(vid, d, x + c[0], y + c[1], z + c[2]);
+        q[j] = cell.x + r3g_mc_dual_patch[12 * (cell.y & 0xffff) + c[3]];
+      }
+      if (!up) { const int t = q[1]; q[1] = q[3]; q[3] = t; }
+      const bool d13 = dual_dist2(verts, q[1], q[3]) < dual_dist2(verts, q[0], q[2]);
+      const int t0[3] = {q[0], q[1], d13 ? q[3] : q[2]};
+      const int t1[3] = {d13 ? q[1] : q[0], q[2], q[3]};
+#pragma unroll
+      for (int i = 0; i < 3; ++i) faces[fo + i] = t0[i];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) faces[fo + 3 + i] = t1[i];
+      fo += 6;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kThreads) mc_case_kernel(const float* __restrict__ g, McDims d, float level,
                                                            unsigned char* __restrict__ out) {
   const int64_t cell = (int64_t)blockIdx.x * kThreads + threadIdx.x;
@@ -680,10 +839,13 @@ extern "C" size_t r3g_mc_workspace_bytes(int n0, int n1, int n2) {
   return carve_sizes(n0, n1, n2, w, nullptr);
 }
 
-extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, void* workspace,
-                            size_t workspace_bytes, int64_t* nv_host, int64_t* nf_host, void* stream) {
+extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, int method,
+                            void* workspace, size_t workspace_bytes, int64_t* nv_host, int64_t* nf_host, void* stream) {
   R3G_ENTRY(ctx, "mc_count");
   if (!grid || !nv_host || !nf_host) return r3g_fail(ctx, R3G_E_INVALID, "mc_count: null argument");
+  if (method != R3G_MC_LEWINER && method != R3G_MC_DUAL)
+    return r3g_fail(ctx, R3G_E_INVALID, "mc_count: unknown method %d", method);
+  const bool dual = method == R3G_MC_DUAL;
   cudaStream_t s = (cudaStream_t)stream;
   McDims d;
   McWorkspace w;
@@ -703,7 +865,12 @@ extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int
   mc_compact_kernel<<<w.seg_blocks, kThreads, 0, s>>>(w.act, d, w.seg_off, w.list);
   R3G_LAUNCH_OK(ctx);
   // from here on the number of crossed cells stays on the device (totals[4]): machine-sized grids walk the list
-  mc_eval_kernel<<<list_grid(ctx, 4), kThreads, 0, s>>>(grid, d, level, w.list, w.totals, w.info, w.cell_counts);
+  if (dual)
+    mc_eval_kernel<true><<<list_grid(ctx, 4), kThreads, 0, s>>>(grid, d, level, w.list, w.totals, w.info,
+                                                                w.cell_counts);
+  else
+    mc_eval_kernel<false><<<list_grid(ctx, 4), kThreads, 0, s>>>(grid, d, level, w.list, w.totals, w.info,
+                                                                 w.cell_counts);
   R3G_LAUNCH_OK(ctx);
   mc_scan2_kernel<<<1, 1024, 0, s>>>(w.cell_counts, w.cell_off, w.totals);
   R3G_LAUNCH_OK(ctx);
@@ -712,7 +879,7 @@ extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int
   *nv_host = ctx->pinned[0];
   *nf_host = ctx->pinned[1];
   const float vmin = ord2f((unsigned)ctx->pinned[2]), vmax = ord2f((unsigned)ctx->pinned[3]);
-  if (!(level >= vmin && level <= vmax)) {
+  if (!dual && !(level >= vmin && level <= vmax)) {
     *nv_host = *nf_host = 0;
     return r3g_fail(ctx, R3G_E_LEVEL, "Surface level must be within volume data range. (level %g, range [%g, %g])",
                     level, vmin, vmax);
@@ -721,11 +888,15 @@ extern "C" int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int
   return R3G_OK;
 }
 
-extern "C" int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level,
+extern "C" int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, int method,
                               const double* bounds_host, void* workspace, size_t workspace_bytes, float* verts,
                               int32_t* faces, void* stream) {
   R3G_ENTRY(ctx, "mc_extract");
   if (!grid || !verts || !faces) return r3g_fail(ctx, R3G_E_INVALID, "mc_extract: null argument");
+  if (method != R3G_MC_LEWINER && method != R3G_MC_DUAL)
+    return r3g_fail(ctx, R3G_E_INVALID, "mc_extract: unknown method %d", method);
+  if (method == R3G_MC_DUAL && bounds_host)
+    return r3g_fail(ctx, R3G_E_INVALID, "mc_extract: the dual method takes no bounds (its vertices are in [0, 1])");
   cudaStream_t s = (cudaStream_t)stream;
   McDims d;
   McWorkspace w;
@@ -733,6 +904,14 @@ extern "C" int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, i
   if (rc) return rc;
   rc = carve(ctx, d, workspace, workspace_bytes, w);
   if (rc) return rc;
+  if (method == R3G_MC_DUAL) {
+    mc_dual_vertex_kernel<<<list_grid(ctx, 4), kThreads, 0, s>>>(grid, d, level, w.list, w.totals, w.info, w.cell_off,
+                                                                 w.vid, verts);
+    R3G_LAUNCH_OK(ctx);
+    mc_dual_face_kernel<<<list_grid(ctx, 8), kThreads, 0, s>>>(d, w.list, w.totals, w.cell_off, w.vid, verts, faces);
+    R3G_LAUNCH_OK(ctx);
+    return R3G_OK;
+  }
   Rescale rs;
   rs.enabled = bounds_host != nullptr;
   const int nax[3] = {n0, n1, n2};

@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libr3g.so")
 
 R3G_OK, R3G_E_INVALID, R3G_E_CUDA, R3G_E_WORKSPACE, R3G_E_LEVEL, R3G_E_NOSURFACE = 0, -1, -2, -3, -4, -5
+R3G_MC_LEWINER, R3G_MC_DUAL = 0, 1
 ATTN_MAX_WINDOWS = 2     # R3G_ATTN_MAX_WINDOWS
 
 
@@ -59,8 +60,8 @@ SIGNATURES = {
     "r3g_last_error": (C.c_char_p, [_vp]),
     "r3g_launch_count": (_i64, [_vp]),
     "r3g_mc_workspace_bytes": (_sz, [_i, _i, _i]),
-    "r3g_mc_count": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _sz, C.POINTER(_i64), C.POINTER(_i64), _vp]),
-    "r3g_mc_extract": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "r3g_mc_count": (_i, [_vp, _vp, _i, _i, _i, _f, _i, _vp, _sz, C.POINTER(_i64), C.POINTER(_i64), _vp]),
+    "r3g_mc_extract": (_i, [_vp, _vp, _i, _i, _i, _f, _i, _vp, _vp, _sz, _vp, _vp, _vp]),
     "r3g_mc_classify": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp]),
     "r3g_mesh_components": (_i, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "r3g_decimate_workspace_bytes": (_sz, [_i64, _i64]),

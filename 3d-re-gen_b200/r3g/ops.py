@@ -486,6 +486,17 @@ def _workspace(kind, device, nbytes):
 def marching_cubes(grid, level=0.0, bounds=None):
     """grid: CUDA float32 [n0,n1,n2].  Returns (verts float32 [V,3], faces int32 [F,3]) CUDA tensors in
     skimage's output convention.  Raises ValueError / RuntimeError like skimage.measure.marching_cubes."""
+    return _extract_surface(grid, level, _abi.R3G_MC_LEWINER, bounds)
+
+
+def dual_marching_cubes(grid):
+    """r3g's dual marching cubes at level 0 (include/r3g.h, R3G_MC_DUAL): grid CUDA float32 [n0,n1,n2] of logits.
+    Returns (verts float32 [V,3] in [0, 1]^3, array-axis order; faces int32 [F,3] with normals towards increasing
+    values) CUDA tensors.  Raises RuntimeError when no cell is crossed."""
+    return _extract_surface(grid, 0.0, _abi.R3G_MC_DUAL, None)
+
+
+def _extract_surface(grid, level, method, bounds):
     if grid.dtype != torch.float32 or grid.dim() != 3:
         raise TypeError("grid must be float32 [n0,n1,n2]")
     grid = grid.contiguous()
@@ -494,7 +505,7 @@ def marching_cubes(grid, level=0.0, bounds=None):
     ws = _workspace("mc", grid.device, ws_bytes)
     nv, nf = C.c_int64(0), C.c_int64(0)
     try:
-        _launch("mc_count", grid, grid, n0, n1, n2, float(level), ws, ws_bytes, C.byref(nv), C.byref(nf))
+        _launch("mc_count", grid, grid, n0, n1, n2, float(level), method, ws, ws_bytes, C.byref(nv), C.byref(nf))
     except _abi.R3GError as e:
         if e.code == _abi.R3G_E_LEVEL:
             raise ValueError("Surface level must be within volume data range.") from None
@@ -506,14 +517,16 @@ def marching_cubes(grid, level=0.0, bounds=None):
     q = 32 << 20
     cap_v = (-(-(nv.value * 12) // q) * q) // 12 + 1
     cap_f = (-(-(nf.value * 12) // q) * q) // 12 + 1
-    verts = torch.empty(cap_v, 3, device=grid.device, dtype=torch.float32)[:nv.value]
-    faces = torch.empty(cap_f, 3, device=grid.device, dtype=torch.int32)[:nf.value]
+    # the library gets the whole buffers: a dual mesh of a grid without interior edges has no face, and an empty slice
+    # would pass a null address
+    verts = torch.empty(cap_v, 3, device=grid.device, dtype=torch.float32)
+    faces = torch.empty(cap_f, 3, device=grid.device, dtype=torch.int32)
     bptr = C.c_void_p(0)
     if bounds is not None:
         barr = (C.c_double * 6)(*[float(v) for v in bounds])
         bptr = C.cast(barr, C.c_void_p)
-    _launch("mc_extract", grid, grid, n0, n1, n2, float(level), bptr, ws, ws_bytes, verts, faces)
-    return verts, faces
+    _launch("mc_extract", grid, grid, n0, n1, n2, float(level), method, bptr, ws, ws_bytes, verts, faces)
+    return verts[:nv.value], faces[:nf.value]
 
 
 def mesh_components(faces, num_vertices):

@@ -6,7 +6,12 @@
   vae.volume_decoder(latents, geo_decoder, ...)  VanillaVolumeDecoder        volume_decoders.py:141-182
   vae.geo_decoder(queries=, latents=)            CrossAttentionDecoder       attention_blocks.py:484-494
   vae.surface_extractor(grid_logits, ...)        MCSurfaceExtractor          surface_extractors.py:50-76
+                                                 DMCSurfaceExtractor         surface_extractors.py:79-94
   SurfaceExtractors registry                                                  surface_extractors.py:97-100
+
+Both extractors run on the GPU.  'mc' is Lewiner marching cubes in scikit-image's conventions.  'dmc' is r3g's own
+dual marching cubes (one vertex per connected patch of a cell's Lewiner tiling, one quad per interior sign-changing grid
+edge; include/r3g.h), not diso's DiffDMC, whose vertex rule and output order are not reproduced.
 
 The encoder side (PointCrossAttentionEncoder, pre_kl) is not on the inference path (SURVEY.md section 2, row 12).
 """
@@ -412,9 +417,27 @@ class MCSurfaceExtractor(SurfaceExtractor):
         return v.cpu().numpy(), np.ascontiguousarray(f.cpu().numpy())
 
 
+def center_vertices(vertices):
+    """surface_extractors.py:29-34: translate the vertices so that their bounding box is centred at zero."""
+    return vertices - 0.5 * (vertices.min(dim=0)[0] + vertices.max(dim=0)[0])
+
+
 class DMCSurfaceExtractor(SurfaceExtractor):
+    """surface_extractors.py:79-94 on r3g's own dual marching cubes (ops.dual_marching_cubes) instead of diso.DiffDMC:
+    the iso value is 0 of the logits, mc_level and bounds are ignored, the vertices are normalised to [0, 1] by
+    (n_axis - 1) and then centred, so the mesh is unit-sized and not in the bounds' frame.  Faces come back with normals
+    towards increasing logits, the winding of MCSurfaceExtractor, so export_to_trimesh makes both outward."""
+
+    keep_on_device = False
+
     def run(self, grid_logit, *, octree_resolution, **kwargs):
-        raise ImportError("Please install diso via `pip install diso`, or set mc_algo to 'mc'")
+        if grid_logit.dtype != torch.float32:      # FlashVDM returns the latents' dtype (fp16) with NaN outside the band
+            grid_logit = grid_logit.float()
+        v, f = ops.dual_marching_cubes(grid_logit)
+        v = center_vertices(v)
+        if self.keep_on_device:
+            return v, f
+        return v.cpu().numpy(), np.ascontiguousarray(f.cpu().numpy())
 
 
 SurfaceExtractors = {"mc": MCSurfaceExtractor, "dmc": DMCSurfaceExtractor}

@@ -55,11 +55,29 @@ int64_t r3g_launch_count(r3g_ctx* ctx);
  *            257^3, 3.0 GB at 513^3; sized for the worst case of every cell crossed), contents need not be
  *            initialised; the same workspace must be passed to count and extract.
  * Limits: (n0-1)*(n1-1)*ceil((n2-1)/32) < 2^27 (about 1600^3), else R3G_E_INVALID.
+ *
+ * method: R3G_MC_LEWINER is the marching cubes above.  R3G_MC_DUAL is r3g's own dual marching cubes, the surface
+ * extractor behind DMCSurfaceExtractor.run (surface_extractors.py:79-94, which calls diso.DiffDMC on -grid / R; diso's
+ * vertex rule, quad split and output order are not reproduced).  Same count / extract protocol and workspace:
+ *   - a point is above iff v > level (NaN is not), and each crossed cell takes the Lewiner tiling chosen above;
+ *   - each connected component ("patch") of that tiling's triangles (joined through shared edge vertices and the
+ *     centre vertex) gives one vertex: the mean of the crossings p_a + t (p_b - p_a), t = v_a / (v_a - v_b), on the
+ *     patch's cube edges, summed in increasing edge order, divided by (n_axis - 1): float64 with explicit rounding,
+ *     stored float32 in array-axis order, so the mesh lies in [0, 1]^3.  Vertices follow the crossed cells in
+ *     traversal order, patches within a cell by their smallest cube edge;
+ *   - each sign-changing grid edge whose four incident cells lie in the grid gives one quad over their four patch
+ *     vertices, wound with its normal towards increasing values (the Lewiner method's winding), split along the
+ *     shorter diagonal (squared float64 lengths; a tie takes vertices 0-2) into two consecutive triangles.  Quads follow
+ *     their owner cell (the first of the four) in traversal order, then the edge's array axis 0, 1, 2.  Edges on the
+ *     grid's outer faces give none, so a surface that reaches the boundary is open there.
+ *   r3g_mc_count returns R3G_E_NOSURFACE when no cell is crossed and applies no level-range check; r3g_mc_extract
+ *   requires bounds_host == NULL (R3G_E_INVALID otherwise).  Any other method is R3G_E_INVALID.
  */
+enum { R3G_MC_LEWINER = 0, R3G_MC_DUAL = 1 };
 size_t r3g_mc_workspace_bytes(int n0, int n1, int n2);
-int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, void* workspace,
+int r3g_mc_count(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, int method, void* workspace,
                  size_t workspace_bytes, int64_t* nv_host, int64_t* nf_host, void* stream);
-int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level,
+int r3g_mc_extract(r3g_ctx* ctx, const float* grid, int n0, int n1, int n2, float level, int method,
                    const double* bounds_host, void* workspace, size_t workspace_bytes, float* verts,
                    int32_t* faces, void* stream);
 /* Per-cell base case 0..14 (Lewiner's `cases[cubeindex][0]`), uint8 [(n0-1)*(n1-1)*(n2-1)]; parity probe. */

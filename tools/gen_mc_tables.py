@@ -355,6 +355,32 @@ def stored(lp):
     return [lp[0]] + lp[:0:-1]
 
 
+DUAL_NO_PATCH = 255
+
+
+def dual_patches(tris):
+    """Dual marching cubes: the connected components ("patches") of one tiling's triangles, joined through shared
+    vertices (cube edges and the centre vertex 12).  Returns (patch of each of the 12 cube edges, DUAL_NO_PATCH for an
+    edge the tiling does not use; number of patches), patches numbered in increasing order of their smallest edge."""
+    par = list(range(13))
+
+    def find(a):
+        while par[a] != a:
+            par[a] = par[par[a]]
+            a = par[a]
+        return a
+    used = set()
+    for t in tris:
+        used.update(t)
+        for v in t[1:]:
+            par[find(v)] = find(t[0])
+    patch, ids = [DUAL_NO_PATCH] * 12, {}
+    for e in range(12):
+        if e in used:
+            patch[e] = ids.setdefault(find(e), len(ids))
+    return patch, len(ids)
+
+
 def mc_case(ci):
     """Lorensen/Chernyaev/Lewiner base-case number 0..14 of a cube index (shape invariant)."""
     def shape(bits):
@@ -538,6 +564,16 @@ def main(out_path):
             for axes in ((lo,), (lo, hi), (hi,)):
                 sl.extend((flip(pu, axes), flip(pw, axes)))
         arr("unsigned char", "r3g_mc_slice", sl, per=6)
+        # dual marching cubes: per tiling, the patch (connected component of its triangles) of each cube edge, numbered
+        # by smallest edge, 255 = edge not crossed; and the number of patches = the vertices the cell gives
+        dual_patch, dual_npatch = [], []
+        for til in range(ntil):
+            tt = tri[tiling_start[til]:tiling_start[til + 1]]
+            p, n = dual_patches([tt[k:k + 3] for k in range(0, len(tt), 3)])
+            dual_patch.extend(p)
+            dual_npatch.append(n)
+        arr("unsigned char", "r3g_mc_dual_patch", dual_patch, per=12)
+        arr("unsigned char", "r3g_mc_dual_npatch", dual_npatch)
         w("#endif\n")
     print(f"tilings={ntil} (tunnel {ntil - n_face_tilings}) tri_entries={len(tri)} max_tris={max_tris}", file=sys.stderr)
 
