@@ -14,7 +14,16 @@ faces...] as int32 words, with the capacity agreed across ranks, so rank 0 posts
     lands it through a pinned ring on a consumer thread.  bench.py's e2e arm uses it at N = 1.
 
 There is no compute kernel to fuse this with: the payload is a few MB per object, after the last kernel.
+
+Object groups split ONE object over G ranks (a torch.distributed process group; member 0, the lowest global rank, is
+the leader): the CFG pair's two DiT forwards run on members 0 and 1, and the dense decode's query chunks are shared
+out over all members (Hunyuan3DDiTFlowMatchingPipeline.__call__'s `object_group=`).  `plan_object_groups` decides which
+objects run that way: the tail of K objects on W ranks that would otherwise leave W - K mod W ranks idle.  The helpers
+below also run on gloo (CPU tensors, or CUDA tensors staged through host memory, which is all gloo's point-to-point
+path carries).
 """
+from dataclasses import dataclass
+
 import torch
 import torch.distributed as dist
 
@@ -303,3 +312,140 @@ class MeshStreamGatherer:
         if self.cuda:
             self.side.synchronize()
         return [self.results[k] for k in sorted(self.results, key=lambda k: (k[1], k[0]))]
+
+
+# ------------------------------------------------------------------------------------------------ object groups
+@dataclass(frozen=True)
+class ObjectGroupPlan:
+    """Which ranks work on which object.  assignments[j] = (object index, global ranks, sorted): one rank for the
+    objects of the full waves, a group of W // T ranks for each of the T = K mod W tail objects."""
+    n_objects: int
+    world: int
+    assignments: tuple
+
+    def for_rank(self, rank):
+        """[(object index, ranks)] that `rank` takes part in, in the order every rank processes them."""
+        return [(i, ranks) for i, ranks in self.assignments if rank in ranks]
+
+    def groups(self):
+        """The rank tuples of the multi-rank groups, in the order their process groups are created."""
+        return [ranks for _, ranks in self.assignments if len(ranks) > 1]
+
+
+def plan_object_groups(n_objects, world):
+    """Deterministic plan (every rank computes the same one from (K, W) alone): the first K - K mod W objects keep the
+    one-object-per-rank assignment of shard_indices (object i on rank i % W); the T = K mod W tail objects, which
+    would run as a last wave on T ranks while W - T wait, each get the G = W // T consecutive ranks [j G, (j + 1) G)."""
+    if n_objects < 0 or world < 1:
+        raise ValueError(f"plan_object_groups: need K >= 0 and W >= 1, got K = {n_objects}, W = {world}")
+    tail = n_objects % world
+    full = n_objects - tail
+    asg = [(i, (i % world,)) for i in range(full)]
+    if tail:
+        g = world // tail
+        asg += [(full + j, tuple(range(j * g, (j + 1) * g))) for j in range(tail)]
+    return ObjectGroupPlan(n_objects, world, tuple(asg))
+
+
+def create_object_groups(plan):
+    """{ranks: ProcessGroup} for the plan's multi-rank groups.  dist.new_group is collective over the whole world, so
+    every rank calls this once with the same plan and the groups are created in the same order everywhere."""
+    if not plan.groups():
+        return {}
+    if not dist.is_initialized():
+        raise RuntimeError("object groups of more than one rank need an initialised torch.distributed world")
+    return {ranks: dist.new_group(list(ranks)) for ranks in plan.groups()}
+
+
+def group_layout(group):
+    """(member index, global ranks of the members) of this process in `group`; (0, (0,)) for None."""
+    if group is None:
+        return 0, (0,)
+    return dist.get_rank(group), tuple(dist.get_process_group_ranks(group))
+
+
+def chunk_ranges(n_chunks, members):
+    """Balanced contiguous shares of n_chunks chunks: [(c0, c1)] per member, sizes differing by at most one; members
+    beyond the chunk count get empty ranges."""
+    b = [m * n_chunks // members for m in range(members + 1)]
+    return [(b[m], b[m + 1]) for m in range(members)]
+
+
+def _p2p(transfers, group):
+    """transfers: [(dist.isend | dist.irecv, tensor, peer global rank)], posted as one batch and waited for (NCCL: the
+    current stream waits; gloo: the host does).  gloo's point-to-point path carries host memory only, so a CUDA tensor
+    travels through a host copy there; on NCCL every tensor is sent / received in place."""
+    if not transfers:
+        return
+    host = dist.get_backend(group) == "gloo"
+    ops_, landed = [], []
+    for op, t, peer in transfers:
+        buf = t
+        if host and t.is_cuda:
+            buf = t.cpu() if op is dist.isend else torch.empty(t.shape, dtype=t.dtype)
+            if op is dist.irecv:
+                landed.append((t, buf))
+        ops_.append(dist.P2POp(op, buf, peer, group))
+    for w in dist.batch_isend_irecv(ops_):
+        w.wait()
+    for t, buf in landed:
+        t.copy_(buf)
+
+
+def exchange_cfg_pair(v_local, v_pair, group):
+    """The per-step exchange of a CFG pair split over members 0 (cond) and 1 (uncond): the all-gather of both samples'
+    model outputs into v_pair [2, ...], ordered (cond, uncond) -- this member's own output is copied into its half, the
+    peer's lands in the other half straight from the wire.  Members >= 2 do not take part."""
+    m, ranks = group_layout(group)
+    if m > 1:
+        raise ValueError("exchange_cfg_pair: only members 0 and 1 hold a CFG sample")
+    v_pair[m].copy_(v_local.view(v_pair[m].shape))
+    _p2p([(dist.isend, v_pair[m], ranks[1 - m]), (dist.irecv, v_pair[1 - m], ranks[1 - m])], group)
+    return v_pair
+
+
+def broadcast_from_leader(t, group, skip_pair=False):
+    """The leader's `t` to the other members, in place.  skip_pair: member 1 already holds the same values (it ran the
+    other half of the CFG pair and the same update), so only members >= 2 receive."""
+    m, ranks = group_layout(group)
+    first = 2 if skip_pair else 1
+    if m == 0:
+        _p2p([(dist.isend, t, r) for r in ranks[first:]], group)
+    elif m >= first:
+        _p2p([(dist.irecv, t, ranks[0])], group)
+    return t
+
+
+def gather_flat_slices(flat, spans, group):
+    """Member m computed flat[spans[m][0]:spans[m][1]] of a flat buffer that every member allocates alike; the leader
+    receives each other member's slice straight into the same slice of its own buffer (no staging copy on NCCL).
+    Empty slices send nothing."""
+    m, ranks = group_layout(group)
+    if m == 0:
+        xfer = [(dist.irecv, flat[s0:s1], ranks[r]) for r, (s0, s1) in enumerate(spans) if r > 0 and s1 > s0]
+    else:
+        s0, s1 = spans[m]
+        xfer = [(dist.isend, flat[s0:s1], ranks[0])] if s1 > s0 else []
+    _p2p(xfer, group)
+    return flat
+
+
+def check_same_inputs(group, *tensors):
+    """Raises unless every member holds bit-identical `tensors` (one all-reduce of a position-weighted checksum of their
+    bits).  A group computes ONE object: members with different seeds or images would otherwise put together a mesh
+    from pieces of different objects."""
+    sums = []
+    for t in tensors:
+        bits = t.detach().contiguous().view(-1)
+        bits = bits.view(torch.int16 if bits.element_size() == 2 else torch.int32).to(torch.int64)
+        pos = torch.arange(bits.numel(), device=bits.device, dtype=torch.int64) % 65521 + 1
+        sums += [bits.sum(), (bits * pos).sum()]
+    c = torch.stack(sums)
+    if dist.get_backend(group) == "gloo":
+        c = c.cpu()
+    both = torch.cat([c, -c])           # max(c) == c and max(-c) == -c on every member iff all c agree
+    dist.all_reduce(both, op=dist.ReduceOp.MAX, group=group)
+    if not torch.equal(both.cpu(), torch.cat([c, -c]).cpu()):
+        m, ranks = group_layout(group)
+        raise RuntimeError(f"object group {list(ranks)}: member {m} holds other inputs (initial latents or condition) "
+                           "than the others; every member must call the pipeline with the same image and seed")

@@ -184,12 +184,15 @@ class Hunyuan3DDiT:
         guidance: [B] fp16, the guidance scale of each sample; required by (and only read by) a guidance-distilled model
         (guidance_embed), which adds guidance_in(timestep_embedding(guidance)) to the time embedding.
 
-        uncond_txt_shared: B == 2 (cond, uncond) and every text row of contexts['main'][1] is the same vector.  t is the
-        same for both samples too, so those Lt rows stay equal through every block (all ops but attention are
-        row-wise, and equal queries see equal keys): batch 1 then runs its GEMMs and attention queries on the window
-        [Lt - 1, L) of live rows -- one representative text row plus the latents.  Attention still sees all L keys:
-        r3g_attention copies the representative row's k / v over the other Lt - 1 text rows first.  Every row is
-        computed as on the full path, so the output is the same bit for bit."""
+        uncond_txt_shared: the last sample of the batch is the unconditional one -- B == 2 (cond, uncond), or B == 1, a
+        lone unconditional sample (one member of a CFG pair split over two GPUs) -- and every text row of its context
+        is the same vector.  Its t is the same at every row too, so those Lt rows stay equal through every block (all
+        ops but attention are row-wise, and equal queries see equal keys): that sample then runs its GEMMs and
+        attention queries on the window [Lt - 1, L) of live rows -- one representative text row plus the latents.
+        Attention still sees all L keys: r3g_attention copies the representative row's k / v over the other Lt - 1 text
+        rows first.  Every row is computed as on the full path, so the output is the same bit for bit, and a lone
+        conditional forward (B = 1, full path) next to a lone collapsed unconditional one gives the two halves of the
+        B = 2 output."""
         if self.w is None:
             raise RuntimeError("Hunyuan3DDiT: no weights loaded")
         w = self.w
@@ -198,8 +201,8 @@ class Hunyuan3DDiT:
         Lt = cond.shape[1]
         L = Li + Lt
         H, Mh, nh = self.hidden_size, self.mlp_hidden, self.num_heads
-        if uncond_txt_shared and B != 2:
-            raise ValueError(f"uncond_txt_shared needs the (cond, uncond) batch of 2, got B = {B}")
+        if uncond_txt_shared and B not in (1, 2):
+            raise ValueError(f"uncond_txt_shared needs the (cond, uncond) batch of 2 or a lone uncond sample, got B = {B}")
         if self.guidance_embed and guidance is None:
             raise ValueError("Didn't get guidance strength for guidance distilled model.")   # hunyuan3ddit.py:394-395
         ws = self._workspace(B, Li, Lt)
@@ -224,12 +227,16 @@ class Hunyuan3DDiT:
 
         q4 = QKV.view(B, L, 3, nh, 64)
         streams = (("img", img, Lt, Li), ("txt", txt, 0, Lt))
-        # the GEMM problems of a double block: (stream, batches, first row, rows).  Collapsed, batch 1's text is its
-        # representative row Lt - 1 alone (rows [0, Lt - 1) of batch 1 are dead: nothing whose output is used reads them,
-        # except their k / v, which attention fills with row Lt - 1's before it reads them)
+        # the GEMM problems of a double block: (stream, batches, first row, rows).  Collapsed, the unconditional
+        # sample's text is its representative row Lt - 1 alone (its rows [0, Lt - 1) are dead: nothing whose output is
+        # used reads them, except their k / v, which attention fills with row Lt - 1's before it reads them)
+        u = B - 1     # the unconditional sample when collapsed
         if uncond_txt_shared:
-            probs = (("img", slice(None), Lt, Li), ("txt", slice(0, 1), 0, Lt), ("txt", slice(1, 2), Lt - 1, 1))
-            windows = ((0, L, 1), (Lt - 1, Li + 1, Lt))
+            probs = (("img", slice(None), Lt, Li),) + ((("txt", slice(0, 1), 0, Lt),) if B == 2 else ()) + (
+                ("txt", slice(u, u + 1), Lt - 1, 1),)
+            windows = ((0, L, 1),) * u + ((Lt - 1, Li + 1, Lt),)
+            # the single blocks' problems: (batch, first row, rows)
+            rows1 = ((0, 0, L),) * u + ((u, Lt - 1, Li + 1),)
         else:
             probs = (("img", slice(None), Lt, Li), ("txt", slice(None), 0, Lt))
             windows = None
@@ -284,17 +291,16 @@ class Hunyuan3DDiT:
             if self.fuse_qk_norm:
                 l1["qk_norm"] = dict(mode=ops.QKN_RMS, q_col0=0, k_col0=H + Mh, cols=H, eps=1e-6, q_w=qs, k_w=ks)
             l2 = dict(w=w[p + "linear2.weight"], bias=w[p + "linear2.bias"])
-            if uncond_txt_shared:   # batch 0's rows and batch 1's live window [Lt - 1, L), one launch each
-                ops.linear_pair(dict(x=XM[0], out=S1[0], **l1), dict(x=XM[1, Lt - 1:], out=S1[1, Lt - 1:], **l1))
+            if uncond_txt_shared:   # the cond sample's rows and the uncond sample's live window [Lt - 1, L), one launch
+                ops.linear_group(*[dict(x=XM[b, r0:r0 + n], out=S1[b, r0:r0 + n], **l1) for b, r0, n in rows1])
             else:
                 ops.linear(XM, out=S1, **l1)
             if not self.fuse_qk_norm:
                 ops.qk_norm_(S1, nh, 0, H + Mh, 64, 0, 1e-6, qs, None, ks, None)
             ops.attention(s1q, s1k, s1v, out=s1q, windows=windows)
             if uncond_txt_shared:
-                ops.linear_pair(dict(x=S1[0, :, :H + Mh], out=X[0], gate=gate[0:1], gate_rows=L, residual=X[0], **l2),
-                                dict(x=S1[1, Lt - 1:, :H + Mh], out=X[1, Lt - 1:], gate=gate[1:2], gate_rows=Li + 1,
-                                     residual=X[1, Lt - 1:], **l2))
+                ops.linear_group(*[dict(x=S1[b, r0:r0 + n, :H + Mh], out=X[b, r0:r0 + n], gate=gate[b:b + 1], gate_rows=n,
+                                        residual=X[b, r0:r0 + n], **l2) for b, r0, n in rows1])
             else:
                 ops.linear(S1[:, :, :H + Mh], out=X, gate=gate, gate_rows=L, residual=X, **l2)
             self._tap(X, Lt, uncond_txt_shared)
@@ -309,12 +315,12 @@ class Hunyuan3DDiT:
     __call__ = forward
 
     def _tap(self, X, Lt, uncond_txt_shared):
-        """Record the hidden state after a block (parity tests).  Collapsed, batch 1's dead text rows are given the value
-        of its representative row first, so that a tap means the same in both modes."""
+        """Record the hidden state after a block (parity tests).  Collapsed, the uncond sample's dead text rows are given
+        the value of its representative row first, so that a tap means the same in both modes."""
         if self.taps is None:
             return
         if uncond_txt_shared:
-            X[1, :Lt - 1] = X[1, Lt - 1:Lt]
+            X[-1, :Lt - 1] = X[-1, Lt - 1:Lt]
         self.taps.append(X.clone())
 
     # FLOPs of one forward for one sample (SURVEY.md section 8d): used by bench.py's roofline

@@ -28,6 +28,11 @@ class GraphCache:
     def __init__(self, keep_all=False):
         self.keep_all = keep_all
         self.entries = {}
+        self.captures = 0           # graphs captured so far (a replayed key costs none)
+
+    def retain(self, keep):
+        """Drops every entry whose key fails keep(key), with its buffers."""
+        self.entries = {k: e for k, e in self.entries.items() if keep(k)}
 
     def get(self, key, inputs, fn, keep=()):
         """The entry for `key`; if absent, `fn(*static inputs)` is run once as a warm-up (workspaces, lazily set
@@ -48,6 +53,7 @@ class GraphCache:
                 with torch.cuda.graph(graph, stream=side):
                     outputs = fn(*static)
                 entry = GraphEntry(graph, static, outputs, ctx.launches - n0, keep)
+            self.captures += 1
             if not self.keep_all:
                 self.entries.clear()
             self.entries[key] = entry

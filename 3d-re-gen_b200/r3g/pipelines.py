@@ -18,13 +18,14 @@ import struct
 import numpy as np
 import torch
 
+from . import dist as r3g_dist
 from . import ops
 from .conditioner import DinoImageEncoder, SingleImageEncoder
 from .dit import Hunyuan3DDiT
 from .graphs import GraphCache
 from .preprocessors import ImageProcessorV2
 from .scheduler import ConsistencyFlowMatchEulerDiscreteScheduler, FlowMatchEulerDiscreteScheduler
-from .vae import ShapeVAE, SurfaceExtractors
+from .vae import ShapeVAE, SurfaceExtractors, VanillaVolumeDecoder
 
 # Hunyuan3D-2 `hunyuan3d-dit-v2-0/config.yaml` values.  The checkpoint config is downloaded at run time by the
 # reference (utils.py:103-126) and is not in the source tree; these are the code defaults plus the published
@@ -288,24 +289,55 @@ class Hunyuan3DDiTPipeline:
         return latents * getattr(self.scheduler, "init_noise_sigma", 1.0)
 
     def _export(self, latents, output_type="trimesh", box_v=1.01, mc_level=0.0, num_chunks=20000,
-                octree_resolution=256, mc_algo="mc", enable_pbar=True):
+                octree_resolution=256, mc_algo="mc", enable_pbar=True, object_group=None):
+        """VAE forward, volume decode, surface extraction.  With an object group of G > 1 members every member runs
+        the VAE forward and decodes its balanced, contiguous share of the dense decode's query chunks; the leader
+        receives the other shares into its grid and extracts the surface, the other members return [None].  FlashVDM's
+        levels depend on the previous level's logits and are not split: with a group the leader runs the VAE forward,
+        the decode and the extraction alone."""
+        member, ranks = r3g_dist.group_layout(object_group)
+        G = len(ranks)
         if output_type == "latent":
-            return latents
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            return latents if member == 0 else [None]
+        dec = self.vae.volume_decoder
+        split = G > 1 and isinstance(dec, VanillaVolumeDecoder) and latents.shape[0] == 1
+        self.timings.pop("gather_ms", None)
+        if member != 0 and not split:       # nothing of this object's export runs here
+            for k in ("vae_ms", "decode_ms", "mc_ms"):
+                self.timings.pop(k, None)
+            self.last_grid = None
+            return [None]
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
         ev[0].record()
         latents = (1.0 / self.vae.scale_factor * latents).contiguous()
         latents = self.vae(latents)
         ev[1].record()
-        grid = self.vae.volume_decoder(latents, self.vae.geo_decoder, bounds=box_v, num_chunks=num_chunks,
-                                       octree_resolution=octree_resolution, enable_pbar=enable_pbar)
-        ev[2].record()
-        outputs = self.vae.surface_extractor(grid, mc_level=mc_level, bounds=box_v,
-                                             octree_resolution=octree_resolution)
+        kw = dict(bounds=box_v, num_chunks=num_chunks, octree_resolution=octree_resolution, enable_pbar=enable_pbar)
+        if split:
+            geo = self.vae.geo_decoder
+            R = int(octree_resolution)
+            ranges = r3g_dist.chunk_ranges(geo.grid_chunks(R)[1], G)
+            grid = dec(latents, geo, chunks=ranges[member], **kw)
+            ev[2].record()
+            spans = [geo.chunk_span(R, c) for c in ranges]
+            r3g_dist.gather_flat_slices(grid.view(-1), spans, object_group)
+        else:
+            grid = dec(latents, self.vae.geo_decoder, **kw)
+            ev[2].record()
         ev[3].record()
+        outputs = [None]
+        if member == 0:
+            outputs = self.vae.surface_extractor(grid, mc_level=mc_level, bounds=box_v,
+                                                 octree_resolution=octree_resolution)
+        ev[4].record()
         torch.cuda.synchronize()
         self.timings.update(vae_ms=ev[0].elapsed_time(ev[1]), decode_ms=ev[1].elapsed_time(ev[2]),
-                            mc_ms=ev[2].elapsed_time(ev[3]))
+                            mc_ms=ev[3].elapsed_time(ev[4]))
+        if split:
+            self.timings.update(gather_ms=ev[2].elapsed_time(ev[3]))
         self.last_grid = grid
+        if member != 0:
+            return outputs
         if output_type == "trimesh":
             outputs = export_to_trimesh(outputs)
         return outputs
@@ -313,10 +345,13 @@ class Hunyuan3DDiTPipeline:
 
 class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
 
-    def _denoise(self, latents, cond, timesteps, guidance_scale, callback=None, callback_steps=None):
+    def _denoise(self, latents, cond, timesteps, guidance_scale, callback=None, callback_steps=None, object_group=None):
         """pipelines.py:741-759.  Per step: one CUDA graph replay of the DiT forward, then the fused Euler update, which
         also rewrites the model input.  With CFG the forward runs on cat([x, x]) with cat([cond, uncond]) and the update
-        mixes the two predictions first; without (a guidance-distilled model, or guidance_scale < 0) it runs on x."""
+        mixes the two predictions first; without (a guidance-distilled model, or guidance_scale < 0) it runs on x.
+        With an object group of more than one member: _denoise_group."""
+        if object_group is not None and r3g_dist.group_layout(object_group)[1][1:]:
+            return self._denoise_group(latents, cond, timesteps, guidance_scale, object_group)
         B = latents.shape[0]
         n = len(timesteps)
         sig = self.scheduler.step_sigmas()
@@ -374,6 +409,69 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
                          self.scheduler.output(i, x_prev, mixed, x.clone()))   # x is updated in place
         return x
 
+    def _denoise_group(self, latents, cond, timesteps, guidance_scale, group):
+        """The denoising loop of one object on an object group.  With CFG, member 0 runs the conditional sample and
+        member 1 the unconditional one (collapsed to one text row when its context allows, as in _denoise): each step
+        is one graph replay of a B = 1 forward, the exchange of the two [Li, C] outputs into one (cond, uncond) buffer,
+        and on both members the same fused CFG / Euler update as on one GPU, so x stays identical on both.  Without CFG
+        member 0 denoises alone.  Members that hold no sample wait, then receive the final latents from the leader."""
+        member, ranks = r3g_dist.group_layout(group)
+        self.timings.pop("exchange_ms", None)
+        B = latents.shape[0]
+        if B != 1:
+            raise ValueError(f"an object group generates one object per call, got a batch of {B}")
+        n = len(timesteps)
+        sig = self.scheduler.step_sigmas()
+        t16 = (timesteps.to(torch.float16) / self.scheduler.config.num_train_timesteps).to(self.device)
+        dsig = [float((sig[i + 1] - sig[i]).to(torch.float16)) for i in range(n)]
+        do_cfg = cond["main"].shape[0] == 2
+        x = latents.contiguous().clone()
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2 * n)]
+        active = member < (2 if do_cfg else 1)
+        if active:
+            ctx = cond["main"][member:member + 1].contiguous()
+            # the unconditional sample runs on one text row when all its rows are one vector (see _denoise)
+            shared = bool(do_cfg and member == 1 and torch.equal(ctx[0], ctx[0, :1].expand_as(ctx[0])))
+            guidance = None
+            if _guidance_distilled(self.model):
+                guidance = torch.tensor([guidance_scale], dtype=torch.float16).to(self.device)
+            gkw = lambda gs: {} if gs is None else {"guidance": gs}  # noqa: E731
+            t_buf = torch.full((1,), 0.5, device=self.device, dtype=torch.float16)
+            x_in = x
+            g = None
+            if self.use_cuda_graph and self.model.taps is None:
+                g = self._graphs.get((x.shape, ctx.shape, shared),
+                                     (x, t_buf, ctx) + ((guidance,) if guidance is not None else ()),
+                                     lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs},
+                                                                            uncond_txt_shared=shared, **gkw(gs)))
+                x_in, t_buf = g.inputs[:2]
+                x_in.copy_(x)
+                g.inputs[2].copy_(ctx)
+                if guidance is not None:
+                    g.inputs[3].copy_(guidance)
+                    guidance = g.inputs[3]
+            x = x_in            # the Euler update below rewrites the model input in place: no copy per step
+            v_pair = torch.empty((2,) + tuple(x.shape[1:]), device=self.device, dtype=x.dtype) if do_cfg else None
+            for i in range(n):
+                t_buf.copy_(t16[i].expand(1))
+                if g is not None:
+                    g.replay()
+                    self.replayed_launches += g.launches
+                    v = g.outputs
+                else:
+                    v = self.model(x_in, t_buf, {"main": ctx}, uncond_txt_shared=shared, **gkw(guidance))
+                if do_cfg:
+                    ev[2 * i].record()
+                    v = r3g_dist.exchange_cfg_pair(v, v_pair, group)
+                    ev[2 * i + 1].record()
+                ops.cfg_euler_step_(x, v, guidance_scale, dsig[i])
+            x = x.clone()       # the graph's static input is rewritten by the next call
+        r3g_dist.broadcast_from_leader(x, group, skip_pair=do_cfg)
+        if active and do_cfg:
+            torch.cuda.synchronize()
+            self.timings["exchange_ms"] = sum(ev[2 * i].elapsed_time(ev[2 * i + 1]) for i in range(n))
+        return x
+
     @torch.inference_mode()
     def __call__(self, image=None, num_inference_steps=50, timesteps=None, sigmas=None, eta=0.0,
                  guidance_scale=5.0, generator=None, box_v=1.01, octree_resolution=384, mc_level=0.0, mc_algo=None,
@@ -382,6 +480,11 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         callback_steps = kwargs.pop("callback_steps", None)
         cond = kwargs.pop("cond", None)  # precomputed {'main': [2B or B, Lt, C]} skips the image encoder (bench/tests)
         latents = kwargs.pop("latents", None)
+        # a torch.distributed process group whose members generate this ONE object together (r3g/dist.py: object
+        # groups); every member calls with the same arguments, the leader returns the output, the others [None]
+        object_group = kwargs.pop("object_group", None)
+        if object_group is not None and not r3g_dist.group_layout(object_group)[1][1:]:
+            object_group = None     # a group of one is the single-GPU path
         self.set_surface_extractor(mc_algo)
         device, dtype = self.device, self.dtype
         # pipelines.py:708-711: a guidance-distilled model runs without CFG
@@ -401,10 +504,14 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         sigmas = np.linspace(0, 1, num_inference_steps) if sigmas is None else sigmas
         ts, num_inference_steps = retrieve_timesteps(self.scheduler, num_inference_steps, device, sigmas=sigmas)
         latents = self.prepare_latents(batch_size, dtype, device, generator, latents)
-        latents = self._denoise(latents, cond, ts, guidance_scale, callback, callback_steps)
+        if object_group is not None:
+            if callback is not None:
+                raise NotImplementedError("callback= is not supported with an object group")
+            r3g_dist.check_same_inputs(object_group, latents, cond["main"])
+        latents = self._denoise(latents, cond, ts, guidance_scale, callback, callback_steps, object_group=object_group)
         ev[2].record()
         out = self._export(latents, output_type, box_v, mc_level, num_chunks, octree_resolution, mc_algo,
-                           enable_pbar=enable_pbar)
+                           enable_pbar=enable_pbar, object_group=object_group)
         torch.cuda.synchronize()
         self.timings.update(cond_ms=ev[0].elapsed_time(ev[1]), denoise_ms=ev[1].elapsed_time(ev[2]))
         return out

@@ -54,7 +54,7 @@ class CrossAttentionDecoder:
         self.count = 0
         self.chunk_queries = 65536
         self.use_cuda_graph = True
-        self._graphs = GraphCache()
+        self._graphs = GraphCache(keep_all=True)    # the graphs of one grid geometry: see decode_grid
         self.w = None
         self._ws = {}
 
@@ -130,37 +130,66 @@ class CrossAttentionDecoder:
         ops.lnpost_dot(x, w["ln_post.weight"], w["ln_post.bias"], w["output_proj.weight"], w["output_proj.bias"],
                        out_f32, eps=1e-5)
 
-    def _decode_grid_eager(self, latents, bounds6, R, flat=None):
+    def grid_chunks(self, R):
+        """(queries per chunk, number of chunks) of the dense decode of an (R+1)^3 grid: chunk c holds the flat grid
+        points [c * cq, min((c + 1) * cq, (R+1)^3))."""
         total = (R + 1) ** 3
-        if flat is None:
-            flat = torch.empty(total, device=latents.device, dtype=torch.float32)
         cq = min(self.chunk_queries, total)
+        return cq, -(-total // cq)
+
+    def chunk_span(self, R, chunks=None):
+        """The flat grid points [s0, s1) that the chunk range [c0, c1) covers (all of them for chunks=None)."""
+        total = (R + 1) ** 3
+        cq, nc = self.grid_chunks(R)
+        c0, c1 = (0, nc) if chunks is None else chunks
+        if not 0 <= c0 <= c1 <= nc:
+            raise ValueError(f"chunk range [{c0}, {c1}) outside the {nc} chunks of a {R + 1}^3 grid")
+        return min(c0 * cq, total), min(c1 * cq, total)
+
+    def _decode_grid_eager(self, latents, bounds6, R, flat=None, chunks=None):
+        """Logits of the grid points of chunks [c0, c1) into flat, which holds exactly those points."""
+        total = (R + 1) ** 3
+        s0, s1 = self.chunk_span(R, chunks)
+        if flat is None:
+            flat = torch.empty(s1 - s0, device=latents.device, dtype=torch.float32)
+        cq = self.grid_chunks(R)[0]
         ws = self._workspace(cq)
         kv = self._project_kv(latents)
-        for s in range(0, total, cq):
+        for s in range(s0, s1, cq):
             n = min(cq, total - s)
             ops.grid_fourier(ws["emb"][:n], s, n, R, bounds6, self.num_freqs, self.include_pi)
-            self._decode(ws, n, kv, flat[s:s + n])
+            self._decode(ws, n, kv, flat[s - s0:s - s0 + n])
         return flat
 
-    def decode_grid(self, latents, bounds6, R, grid_out):
+    def decode_grid(self, latents, bounds6, R, grid_out, chunks=None):
         """All (R+1)^3 dense-grid logits; queries are generated in-kernel (no [(R+1)^3, 3] list in HBM).
         The whole decode -- K/V projection + ceil((R+1)^3 / 65536) chunks x 10 kernels -- is captured ONCE per
         (R, bounds) into a CUDA graph over static buffers and replayed per object: eager launches left ~10 % of the
         decode idle between kernels (tools/decode_probe.py: 2.61 ms per chunk in a graph, 2.90 ms eager).
-        One (R, bounds) is cached at a time: the graph's grid is (R+1)^3 floats."""
-        total = (R + 1) ** 3
+        One grid geometry (R, bounds, latent shape) is cached at a time, with one graph per chunk range decoded for
+        it: a rank that runs whole objects and also its share of a split one (object groups, r3g/dist.py) replays both
+        graphs instead of capturing them again every time it switches.  The whole decode's graph holds (R+1)^3
+        floats of logits, a chunk range's graph only the logits of its range.
+
+        chunks: optional range [c0, c1) of the chunks above (grid_chunks); only those chunks' logits are computed and
+        written, into the matching slice of the flat grid (chunk_span), the rest of grid_out is not touched.  The
+        chunks are the ones of the whole decode, so every logit comes from a launch of the same shape as there."""
         flat = grid_out.view(-1)
+        s0, s1 = self.chunk_span(R, chunks)
+        if s1 == s0:
+            return grid_out
         if not self.use_cuda_graph or latents.device.type != "cuda":
-            self._decode_grid_eager(latents, bounds6, R, flat)
+            self._decode_grid_eager(latents, bounds6, R, flat[s0:s1], chunks)
         else:
-            key = (int(R), tuple(float(b) for b in bounds6), tuple(latents.shape))
-            g = self._graphs.get(key, (latents,), lambda lat: self._decode_grid_eager(lat, bounds6, R),
-                                 keep=self._workspace(min(self.chunk_queries, total)))
+            geometry = (int(R), tuple(float(b) for b in bounds6), tuple(latents.shape))
+            key = geometry + (None if chunks is None else tuple(int(c) for c in chunks),)
+            self._graphs.retain(lambda k: k[:3] == geometry)     # another grid: its graphs and grids are dropped
+            g = self._graphs.get(key, (latents,), lambda lat: self._decode_grid_eager(lat, bounds6, R, chunks=chunks),
+                                 keep=self._workspace(self.grid_chunks(R)[0]))
             g.inputs[0].copy_(latents)
             g.replay()
-            flat.copy_(g.outputs)
-        self.count += total
+            flat[s0:s1].copy_(g.outputs)
+        self.count += s1 - s0
         return grid_out
 
     def __call__(self, queries=None, query_embeddings=None, latents=None):
@@ -189,11 +218,12 @@ class CrossAttentionDecoder:
 
 class VanillaVolumeDecoder:
     """volume_decoders.py:141-182.  `num_chunks` is accepted for interface parity; chunking here is an
-    internal workspace decision and does not change the result."""
+    internal workspace decision and does not change the result.  `chunks=(c0, c1)` decodes only that range of the
+    geo decoder's query chunks (CrossAttentionDecoder.decode_grid); the rest of the returned grid is uninitialised."""
 
     @torch.no_grad()
     def __call__(self, latents, geo_decoder, bounds=1.01, num_chunks=10000, octree_resolution=None,
-                 enable_pbar=True, **kwargs):
+                 enable_pbar=True, chunks=None, **kwargs):
         if isinstance(bounds, float):
             bounds = [-bounds, -bounds, -bounds, bounds, bounds, bounds]
         R = int(octree_resolution)
@@ -201,7 +231,7 @@ class VanillaVolumeDecoder:
         grid = torch.empty(B, R + 1, R + 1, R + 1, device=latents.device, dtype=torch.float32)
         for b in range(B):
             if isinstance(geo_decoder, CrossAttentionDecoder):
-                geo_decoder.decode_grid(latents[b:b + 1], [float(v) for v in bounds], R, grid[b])
+                geo_decoder.decode_grid(latents[b:b + 1], [float(v) for v in bounds], R, grid[b], chunks=chunks)
             else:
                 raise TypeError("VanillaVolumeDecoder needs the r3g CrossAttentionDecoder")
         return grid

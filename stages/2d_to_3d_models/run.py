@@ -9,7 +9,9 @@ mini, use_all_available_cuda; non-zero exit on failure.
 Differences, all on purpose:
   * one process per GPU (torchrun / torch.distributed, NCCL) instead of a spawn-pool that reloads both models for
     every image (reference run.py:108-133): each rank loads the weights once, takes images i % world == rank of
-    the SORTED list, and the finished meshes are gathered to rank 0 (r3g/dist.py::MeshBatchGatherer, over NCCL
+    the SORTED list -- except the last K mod world images, each of which runs on a group of world // (K mod world)
+    ranks that split its CFG pair and dense decode (r3g/dist.py::plan_object_groups; only the group's leader
+    post-processes and submits that mesh) -- and the finished meshes are gathered to rank 0 (r3g/dist.py::MeshBatchGatherer, over NCCL
     when there is more than one rank), which writes each .glb as its mesh lands;
   * FloaterRemover runs on the GPU (r3g/postprocessors.py: union-find components, MeshLab's 0.5 % rule) and
     DegenerateFaceRemover is the reference's no-op round trip; the face reduction to 40 000 faces is FaceReducerR3G,
@@ -36,7 +38,7 @@ from PIL import Image
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
 
-from r3g.dist import MeshBatchGatherer, shard_indices  # noqa: E402
+from r3g.dist import MeshBatchGatherer, create_object_groups, plan_object_groups  # noqa: E402
 from r3g.pipelines import Hunyuan3DDiTFlowMatchingPipeline, SimpleMesh  # noqa: E402
 from r3g.postprocessors import DegenerateFaceRemover, FaceReducerR3G, FloaterRemover  # noqa: E402
 
@@ -88,16 +90,22 @@ def main():
         pipe = Hunyuan3DDiTFlowMatchingPipeline.from_pretrained(repo, device=f"cuda:{local}", **kw)
     pipe.vae.surface_extractor.keep_on_device = True     # the mesh leaves the GPU once, after the floater removal
 
-    mine = shard_indices(len(names), rank, world)
+    # full waves one object per rank (i % world == rank), the tail objects on rank groups; every rank creates the
+    # process groups, in the same order
+    plan = plan_object_groups(len(names), world)
+    groups = create_object_groups(plan)
     local_meshes, local_names = [], []
-    for i in mine:
+    for i, ranks in plan.for_rank(rank):
         t0 = time.time()
         image = Image.open(os.path.join(input_folder, names[i])).convert("RGBA")
         out = pipe(image=image, num_inference_steps=config.get("num_inf_steps_hy", 100),
                    octree_resolution=config.get("octree_resolution_hy", 380),
                    num_chunks=config.get("num_chunks_hy", 20000),
-                   generator=torch.manual_seed(config.get("seed", 12345)), output_type="mesh")[0]
+                   generator=torch.manual_seed(config.get("seed", 12345)), output_type="mesh",
+                   object_group=groups.get(ranks))[0]
         stem = os.path.splitext(names[i])[0]
+        if rank != ranks[0]:        # a group member other than the leader: the leader holds the mesh
+            continue
         if out is None:
             print(f"[rank {rank}] {stem}: no surface", flush=True)
             continue
@@ -113,6 +121,7 @@ def main():
         print(f"[rank {rank}] {stem}: {v.shape[0]} vertices, {f.shape[0]} faces (reduced from {raw_faces}) in "
               f"{time.time() - t0:.2f} s", flush=True)
 
+    # the names of the meshes each rank submits: its own objects and the groups it leads, in plan order
     all_names = [local_names]
     if world > 1:
         all_names = [None] * world
