@@ -5,7 +5,10 @@ LayerScale) once per object, ~3 TFLOP.  Here `self.model` is still that HF modul
 checkpoint loads into (pipelines.py:179-180 loads it strictly) -- but on a CUDA device the forward runs on the r3g
 kernels (SURVEY.md section 8f row 4): patchify + wgmma GEMM for the 14x14 patch embedding, LayerNorm, one q|k|v
 projection, flash attention, projection with the LayerScale-gated residual fused in the epilogue, SwiGLU gate.
-`backend="hf"` keeps the library forward (CPU, and the parity test's other side)."""
+`backend="hf"` keeps the library forward (CPU, and the parity test's other side).
+DinoImageEncoderMV (conditioner.py:134-200, Hunyuan3D-2mv) runs the same forward on the B * V views of a multi-view
+input and adds a fixed per-view embedding: {'main': [B, V * 1370, 1536]}."""
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -134,17 +137,20 @@ class DinoImageEncoder:
         std = torch.tensor(self.std, device=image.device, dtype=image.dtype)[None, :, None, None]
         return (image - mean) / std
 
-    @torch.no_grad()
-    def __call__(self, image, mask=None, value_range=(-1, 1), **kwargs):
+    def _last_hidden_state(self, image, value_range):
+        """[N, 3, H, W] in value_range -> the model's last_hidden_state [N, 1 + P, C], cls token included."""
         if value_range is not None:
             lo, hi = value_range
             image = (image - lo) / (hi - lo)
         p = next(self.model.parameters())
         image = image.to(p.device, dtype=p.dtype)
         if self.backend == "r3g":
-            hidden = self._forward_r3g(self._transform(image))
-        else:
-            hidden = self.model(self._transform(image)).last_hidden_state
+            return self._forward_r3g(self._transform(image))
+        return self.model(self._transform(image)).last_hidden_state
+
+    @torch.no_grad()
+    def __call__(self, image, mask=None, value_range=(-1, 1), **kwargs):
+        hidden = self._last_hidden_state(image, value_range)
         return hidden if self.use_cls_token else hidden[:, 1:, :]
 
     def unconditional_embedding(self, batch_size, **kwargs):
@@ -152,11 +158,91 @@ class DinoImageEncoder:
         return torch.zeros(batch_size, self.num_patches, self.model.config.hidden_size, device=p.device, dtype=p.dtype)
 
 
+def view_embedding_table(dim, view_num):
+    """The fixed 1-D sin-cos embedding of view indices 0 .. view_num - 1 (get_1d_sincos_pos_embed_from_grid,
+    conditioner.py:37-54): float32 [view_num, dim], columns sin(v * w_i) then cos(v * w_i) with
+    w_i = 1 / 10000^(i / (dim / 2)).  Evaluated in float64 as the reference's numpy code is, then rounded to float32."""
+    if dim % 2:
+        raise ValueError(f"view embedding width must be even, got {dim}")
+    freq = 1.0 / np.power(10000, np.arange(dim // 2, dtype=np.float64) / (dim / 2.0))
+    views = np.arange(view_num, dtype=np.float32).astype(np.float64)
+    ang = views[:, None] * freq[None, :]
+    return np.concatenate([np.sin(ang), np.cos(ang)], axis=1).astype(np.float32)
+
+
+class DinoImageEncoderMV(DinoImageEncoder):
+    """The Hunyuan3D-2mv conditioner (conditioner.py:134-200): image [B, V, 3, H, W] -> [B, V * (1 + P), C].
+
+    The B * V views run through the DINOv2 forward as one batch (on the r3g kernels on a CUDA device), then each view's
+    1 + P tokens get the view embedding of its index added: view_idxs[b] (one tuple of V indices per object, as
+    MVImageProcessorV2 returns them) or, without view_idxs, indices 0 .. V - 1.  The add is one fp16 element-wise op
+    per object in torch, outside the denoising loop.  The table is built once per encoder (view_embedding_table) and is
+    not part of the state dict, as in the reference."""
+
+    def __init__(self, version=None, config=None, use_cls_token=True, image_size=224, view_num=4, device="cuda",
+                 dtype=torch.float16, backend=None, **kwargs):
+        if not use_cls_token:
+            # the reference's forward keeps all 1 + P tokens and its view_embed has num_patches (= P then) rows
+            raise ValueError("DinoImageEncoderMV adds its view embedding to all 1 + P tokens: use_cls_token must be True")
+        super().__init__(version=version, config=config, use_cls_token=use_cls_token, image_size=image_size,
+                         device=device, dtype=dtype, backend=backend, **kwargs)
+        self.view_num = view_num
+        self.view_table = view_embedding_table(self.model.config.hidden_size, view_num)   # float32 numpy
+        self._view_embed = None        # view_table on the model's device in the model's dtype
+
+    def view_embedding(self, num_views, view_idxs=None):
+        """The embeddings added to the views: [B, V, C] for view_idxs (B tuples of V indices), else [1, V, C]."""
+        p = next(self.model.parameters())
+        if self._view_embed is None or self._view_embed.device != p.device or self._view_embed.dtype != p.dtype:
+            # conditioner.py:173/181: the float32 table is cast to the hidden state's dtype before the add
+            self._view_embed = torch.from_numpy(self.view_table).to(p.device).to(p.dtype)
+        if view_idxs is None:
+            if num_views > self.view_num:
+                raise ValueError(f"{num_views} views but a view embedding of {self.view_num}")
+            return self._view_embed[None, :num_views]
+        if any(len(v) != num_views for v in view_idxs):
+            raise ValueError(f"every view_idxs entry must name the {num_views} views of its object, got {list(view_idxs)}")
+        idx = torch.as_tensor([list(v) for v in view_idxs], dtype=torch.long)
+        if idx.numel() and (idx.min() < 0 or idx.max() >= self.view_num):
+            raise IndexError(f"view index outside [0, {self.view_num}): {list(view_idxs)}")
+        return self._view_embed[idx.to(p.device)]
+
+    @torch.no_grad()
+    def __call__(self, image, mask=None, value_range=(-1, 1), view_idxs=None, **kwargs):
+        B, V = image.shape[:2]
+        if view_idxs is not None and len(view_idxs) != B:
+            raise ValueError(f"view_idxs holds {len(view_idxs)} entries for a batch of {B}")
+        hidden = self._last_hidden_state(image.reshape(B * V, *image.shape[2:]), value_range)
+        hidden = hidden.view(B, V, hidden.shape[1], hidden.shape[2])
+        hidden = hidden + self.view_embedding(V, view_idxs)[:, :, None, :]
+        return hidden.view(B, V * hidden.shape[2], hidden.shape[3])
+
+    def unconditional_embedding(self, batch_size, view_idxs=None, **kwargs):
+        """Zeros [B, (1 + P) * V, C] with V = len(view_idxs[0]) (conditioner.py:190-200)."""
+        if view_idxs is None:
+            raise ValueError("the multi-view unconditional embedding needs view_idxs for its number of views")
+        p = next(self.model.parameters())
+        return torch.zeros(batch_size, self.num_patches * len(view_idxs[0]), self.model.config.hidden_size,
+                           device=p.device, dtype=p.dtype)
+
+
+IMAGE_ENCODERS = {"DinoImageEncoder": DinoImageEncoder, "DinoImageEncoderMV": DinoImageEncoderMV}
+
+
+def image_encoder_class(type_name):
+    """The encoder class a config's `main_image_encoder.type` names (conditioner.py:203-211 build_image_encoder)."""
+    if type_name not in IMAGE_ENCODERS:
+        raise NotImplementedError(f"main_image_encoder type {type_name!r}: only {' and '.join(IMAGE_ENCODERS)} are "
+                                  "mirrored")
+    return IMAGE_ENCODERS[type_name]
+
+
 class SingleImageEncoder:
     def __init__(self, main_image_encoder=None, **kwargs):
         self.main_image_encoder = main_image_encoder if main_image_encoder is not None else DinoImageEncoder(**kwargs)
 
     def __call__(self, image, mask=None, **kwargs):
+        # kwargs carries the multi-view processor's view_idxs to the encoder (DinoImageEncoder ignores it)
         return {"main": self.main_image_encoder(image, mask=mask, **kwargs)}
 
     forward = __call__

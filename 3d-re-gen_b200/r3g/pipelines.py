@@ -10,6 +10,9 @@ Everything between the conditioner output and the mesh runs in libr3g.so: 50 x (
 fused CFG/Euler step), ShapeVAE transformer, dense SDF decode, marching cubes.  A guidance-distilled checkpoint
 (`hunyuan3d-dit-v2-0-fast` / `-turbo`: `guidance_embed: true`) runs without CFG, one sample per step with the guidance
 scale as a model input; the `-turbo` config's ConsistencyFlowMatchEulerDiscreteScheduler gives its 5-step schedule.
+A multi-view (Hunyuan3D-2mv) pipeline takes `image={'front': ..., 'left': ..., 'back': ..., 'right': ...}` (any
+subset, any order): MVImageProcessorV2 stacks the views, DinoImageEncoderMV gives a V * 1370-row context, and the
+same DiT runs on it.
 """
 import json
 import os
@@ -20,10 +23,10 @@ import torch
 
 from . import dist as r3g_dist
 from . import ops
-from .conditioner import DinoImageEncoder, SingleImageEncoder
+from .conditioner import SingleImageEncoder, image_encoder_class
 from .dit import Hunyuan3DDiT
 from .graphs import GraphCache
-from .preprocessors import ImageProcessorV2
+from .preprocessors import ImageProcessorV2, MVImageProcessorV2
 from .scheduler import ConsistencyFlowMatchEulerDiscreteScheduler, FlowMatchEulerDiscreteScheduler
 from .vae import ShapeVAE, SurfaceExtractors, VanillaVolumeDecoder
 
@@ -49,6 +52,25 @@ HUNYUAN3D_2_TURBO_CONFIG = dict(
                    num_train_timesteps=1000, pcm_timesteps=100),
 )
 
+# Hunyuan3D-2mv (`hunyuan3d-dit-v2-mv`, and `-mv-fast` / `-mv-turbo` below): up to four views of one object, each
+# encoded by DINOv2 into 1370 tokens plus a per-view embedding, so the DiT's context holds V * 1370 rows.  The DiT and
+# VAE are assumed to be 2.0's: UNVERIFIED, the checkpoints' config.yaml files are downloaded at run time and are not in
+# the reference tree; the model zoo lists the same 1.1 B parameters and the reference pairs 2mv with the 2.0 VAE
+# (pipelines.py:270,291).  view_num = 4 and image_size = 518 (1370 tokens per view) are likewise assumed.
+HUNYUAN3D_2MV_CONFIG = dict(
+    HUNYUAN3D_2_CONFIG,
+    conditioner=dict(type="DinoImageEncoderMV", kwargs=dict(view_num=4, image_size=518, use_cls_token=True)),
+    image_processor=dict(target="hy3dgen.shapegen.preprocessors.MVImageProcessorV2", size=512, border_ratio=0.15),
+)
+
+# `hunyuan3d-dit-v2-mv-turbo`: the multi-view conditioner with the -turbo DiT and scheduler (same UNVERIFIED
+# assumptions as both configs above)
+HUNYUAN3D_2MV_TURBO_CONFIG = dict(
+    HUNYUAN3D_2_TURBO_CONFIG,
+    conditioner=HUNYUAN3D_2MV_CONFIG["conditioner"],
+    image_processor=HUNYUAN3D_2MV_CONFIG["image_processor"],
+)
+
 
 def _guidance_distilled(model):
     """pipelines.py:708-711 / :733-735: `hasattr(model, 'guidance_embed') and model.guidance_embed is True`."""
@@ -64,6 +86,18 @@ def scheduler_class(target):
         return ConsistencyFlowMatchEulerDiscreteScheduler
     raise NotImplementedError(f"scheduler target {target!r}: only FlowMatchEulerDiscreteScheduler and "
                               "ConsistencyFlowMatchEulerDiscreteScheduler (the Hunyuan3D-2 shape checkpoints') are mirrored")
+
+
+def image_processor_class(target):
+    """The image processor a config's `image_processor.target` names (pipelines.py:182 instantiates it).  None: the
+    single-view ImageProcessorV2."""
+    name = None if target is None else str(target).rsplit(".", 1)[-1]
+    if name is None or name == "ImageProcessorV2":
+        return ImageProcessorV2
+    if name == "MVImageProcessorV2":
+        return MVImageProcessorV2
+    raise NotImplementedError(f"image_processor target {target!r}: only ImageProcessorV2 and MVImageProcessorV2 (the "
+                              "Hunyuan3D-2 / -2mv shape checkpoints') are mirrored")
 
 
 class SimpleMesh:
@@ -159,8 +193,9 @@ class Hunyuan3DDiTPipeline:
     def from_random(cls, seed=0, device="cuda", dtype=torch.float16, config=None, conditioner="dinov2",
                     **kwargs):
         """Architecture of tencent/Hunyuan3D-2 `hunyuan3d-dit-v2-0` with seeded random weights (there is no
-        network for checkpoints).  conditioner: "dinov2" (random-init DINOv2-giant through HF transformers) or
-        None (callers then pass precomputed `cond=` tensors)."""
+        network for checkpoints).  conditioner: "dinov2" (random-init DINOv2-giant through HF transformers, of the
+        config's `conditioner` type: DinoImageEncoder when it has none) or None (callers then pass precomputed `cond=`
+        tensors).  The config's `image_processor.target` picks the image processor (image_processor_class)."""
         cfg = config or HUNYUAN3D_2_CONFIG
         model = Hunyuan3DDiT(device=device, **cfg["model"]).init_random(seed)
         vae = ShapeVAE(device=device, **cfg["vae"]).init_random(seed + 1)
@@ -168,10 +203,13 @@ class Hunyuan3DDiTPipeline:
         sched = scheduler_class(sc.pop("target", None))(**sc)
         cond = None
         if conditioner == "dinov2":
+            enc = cfg.get("conditioner", dict(type="DinoImageEncoder", kwargs=dict(image_size=518)))
             torch.manual_seed(seed + 2)
-            cond = SingleImageEncoder(DinoImageEncoder(device=device, dtype=dtype, image_size=518))
+            cond = SingleImageEncoder(image_encoder_class(enc["type"])(device=device, dtype=dtype, **enc["kwargs"]))
+        ip = dict(cfg["image_processor"])
         return cls(vae=vae, model=model, scheduler=sched, conditioner=cond,
-                   image_processor=ImageProcessorV2(**cfg["image_processor"]), device=device, dtype=dtype, **kwargs)
+                   image_processor=image_processor_class(ip.pop("target", None))(**ip), device=device, dtype=dtype,
+                   **kwargs)
 
     @classmethod
     def from_single_file(cls, ckpt_path, config_path, device="cuda", dtype=torch.float16, use_safetensors=None,
@@ -182,6 +220,7 @@ class Hunyuan3DDiTPipeline:
         with open(config_path) as fh:
             config = yaml.safe_load(fh)
         sched_cls = scheduler_class(config["scheduler"].get("target"))
+        proc_cls = image_processor_class(config["image_processor"].get("target"))
         if use_safetensors:
             ckpt_path = ckpt_path.replace(".ckpt", ".safetensors")
         if not os.path.exists(ckpt_path):
@@ -205,13 +244,13 @@ class Hunyuan3DDiTPipeline:
             raise NotImplementedError(f"conditioner target {cc.get('target')!r}: only SingleImageEncoder (the "
                                       "Hunyuan3D-2 shape checkpoints' conditioner) is mirrored")
         enc_cfg = cc["params"]["main_image_encoder"]
-        if enc_cfg.get("type") != "DinoImageEncoder":
-            raise NotImplementedError(f"main_image_encoder type {enc_cfg.get('type')!r}: only DinoImageEncoder is mirrored")
+        enc_cls = image_encoder_class(enc_cfg.get("type"))     # DinoImageEncoder, or DinoImageEncoderMV (2mv)
         enc_kw = dict(enc_cfg.get("kwargs") or {})
         enc_kw.setdefault("image_size", 224)          # ImageEncoder.__init__ default (conditioner.py:62)
-        enc = DinoImageEncoder(device=device, dtype=dtype, **enc_kw)
+        enc = enc_cls(device=device, dtype=dtype, **enc_kw)
         if "conditioner" in ckpt:
-            # conditioner.load_state_dict(ckpt['conditioner']) is strict in the reference (pipelines.py:179-180)
+            # conditioner.load_state_dict(ckpt['conditioner']) is strict in the reference (pipelines.py:179-180); the
+            # multi-view encoder's view_embed is a plain attribute there, not a state-dict entry
             pre = "main_image_encoder.model."
             bad = [k for k in ckpt["conditioner"] if not k.startswith(pre)]
             if bad:
@@ -220,7 +259,7 @@ class Hunyuan3DDiTPipeline:
             enc.invalidate()
         return cls(vae=vae, model=model, scheduler=sched_cls(**config["scheduler"]["params"]),
                    conditioner=SingleImageEncoder(enc),
-                   image_processor=ImageProcessorV2(**config["image_processor"]["params"]), device=device,
+                   image_processor=proc_cls(**config["image_processor"]["params"]), device=device,
                    dtype=dtype, **kwargs)
 
     @classmethod
@@ -262,6 +301,8 @@ class Hunyuan3DDiTPipeline:
         self.vae.surface_extractor = SurfaceExtractors[mc_algo]()
 
     def prepare_image(self, image):
+        """pipelines.py:490-510: image (a path, PIL image or multi-view dict, or a list of them) -> {'image': the
+        processors' tensors concatenated, 'mask': likewise, 'view_idxs': [one tuple per object] (multi-view only)}."""
         if isinstance(image, str) and not os.path.exists(image):
             raise FileNotFoundError(f"Couldn't find image at path {image}")
         images = image if isinstance(image, list) else [image]

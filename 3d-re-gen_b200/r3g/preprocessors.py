@@ -1,5 +1,6 @@
-"""Host-side image preparation, interface of Hunyuan3D-2/hy3dgen/shapegen/preprocessors.py:30-117
-(ImageProcessorV2): alpha-bbox recentre on a white square, cubic resize to `size`, scale to [-1, 1].
+"""Host-side image preparation, interface of Hunyuan3D-2/hy3dgen/shapegen/preprocessors.py:30-159
+(ImageProcessorV2): alpha-bbox recentre on a white square, cubic resize to `size`, scale to [-1, 1];
+MVImageProcessorV2 does that per view of a multi-view dict and stacks the views in index order.
 CPU / OpenCV work done once per object; not a kernel target (SURVEY.md section 8a row a1)."""
 import cv2
 import numpy as np
@@ -67,5 +68,29 @@ class ImageProcessorV2:
         return {"image": img, "mask": mask}
 
 
-IMAGE_PROCESSORS = {"v2": ImageProcessorV2}
+class MVImageProcessorV2(ImageProcessorV2):
+    """Multi-view input of Hunyuan3D-2mv (preprocessors.py:120-159): a dict {view tag: path or PIL image} with tags
+    front (0), left (1), back (2), right (3), i.e. the front view turned clockwise by 0, 90, 180 and 270 degrees.  Each
+    view goes through ImageProcessorV2; the views are ordered by index whatever the dict order, and stacked into
+    image [1, V, 3, S, S], mask [1, V, 1, S, S] plus the sorted `view_idxs` tuple.  An unknown tag raises KeyError."""
+    return_view_idx = True
+    VIEW_INDEX = {"front": 0, "left": 1, "back": 2, "right": 3}
+
+    def __init__(self, size=512, border_ratio=None):
+        super().__init__(size, border_ratio)
+        self.view2idx = dict(self.VIEW_INDEX)
+
+    def __call__(self, image_dict, border_ratio=0.15, to_tensor=True, **kwargs):
+        if self.border_ratio is not None:
+            border_ratio = self.border_ratio
+        views = []
+        for tag, image in image_dict.items():
+            idx = self.view2idx[tag]            # KeyError on an unknown tag, before any image is loaded
+            views.append((idx, *self.load_image(image, border_ratio=border_ratio, to_tensor=to_tensor)))
+        views.sort(key=lambda v: v[0])          # dict keys are distinct, so are their indices
+        idxs, imgs, masks = zip(*views)
+        return {"image": torch.cat(imgs, 0)[None], "mask": torch.cat(masks, 0)[None], "view_idxs": idxs}
+
+
+IMAGE_PROCESSORS = {"v2": ImageProcessorV2, "mv_v2": MVImageProcessorV2}
 DEFAULT_IMAGEPROCESSOR = "v2"
