@@ -557,6 +557,8 @@ int validate_linear(r3g_ctx* ctx, const r3g_linear_args* a) {
     return r3g_fail(ctx, R3G_E_INVALID, "linear: an fp32 output takes an fp32 residual (residual_f32=1) and vice versa");
   if (a->ls_gamma && !a->residual_f32) return r3g_fail(ctx, R3G_E_INVALID, "linear: ls_gamma needs the fp32 residual form");
   if (a->gate && (!a->residual || a->gate_ld % 8)) return r3g_fail(ctx, R3G_E_INVALID, "linear: gate needs residual");
+  if (a->gate && a->residual_f32)
+    return r3g_fail(ctx, R3G_E_INVALID, "linear: gate takes the fp16 residual form, not residual_f32 (use ls_gamma)");
   if (a->act && (a->act_col0 % 32 || a->act_col1 % 32))
     return r3g_fail(ctx, R3G_E_INVALID, "linear: activation column range must be aligned to 32 columns");
   if (a->qkn_mode) {

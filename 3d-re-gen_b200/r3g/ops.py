@@ -129,6 +129,8 @@ def _linear_args(dev, x, w, bias=None, *, out=None, act=ACT_NONE, act_cols=None,
     a.seg_len, a.x_seg_stride, a.y_seg_stride = seg_len, xs, ys
     a.act = act
     a.act_col0, a.act_col1 = act_cols if act_cols is not None else (0, N)
+    if ls_gamma is not None and (residual is None or residual.dtype != torch.float32):
+        raise ValueError("linear: ls_gamma scales the float32-residual form only; pass a float32 residual")
     if gate is not None:
         _f16(gate, "gate")
         a.gate, a.gate_ld, a.gate_rows = _ptr(gate, dev, "linear", "gate"), gate.stride(0), gate_rows
@@ -306,7 +308,7 @@ def gemv(w, bias, vec, silu_in=False, silu_out=False, out=None, residual=None):
 def swiglu(x, F, out=None):
     """out[:, j] = silu(x[:, j]) * x[:, F + j]  (fp16 roundings of Dinov2SwiGLUFFN); x [M, 2F] -> out [M, F]."""
     _f16(x, "x")
-    rows, width, ldx, _, _ = _rows(x, "x")
+    rows, width, ldx, _, _ = _rows(x, "x", segments=False)
     if width < 2 * F:
         raise ValueError("swiglu: x must hold 2F columns")
     out = _out("swiglu", out, (*x.shape[:-1], F), torch.float16, x, rows=True)
@@ -369,8 +371,15 @@ def points_fourier_f32(queries, out, num_freqs, include_pi):
 
 
 def lnpost_dot(x, ln_w, ln_b, w_out, b_out, out, eps=1e-5):
-    """ln_post + output_proj of the geo decoder: one float32 logit per row of x into out, contiguous [rows]."""
-    rows, width, ldx, _, _ = _rows(x, "x")
+    """ln_post + output_proj of the geo decoder: one float32 logit per row of x into out, contiguous [rows].
+    x: fp16 rows with one row stride; ln_w, ln_b, w_out: fp16 [width]; b_out: fp16 [1] or None."""
+    _f16(x, "x")
+    rows, width, ldx, _, _ = _rows(x, "x", segments=False)
+    for t, name in ((ln_w, "ln_w"), (ln_b, "ln_b"), (w_out, "w_out")):
+        if _f16(t, name).numel() != width:
+            raise ValueError(f"lnpost_dot: {name} must hold width = {width} values, got {t.numel()}")
+    if b_out is not None:
+        _f16(b_out, "b_out")
     _out("lnpost_dot", out, (rows,), torch.float32, x, contiguous=True)
     _launch("lnpost_dot", x, x, ldx, rows, width, float(eps), ln_w, ln_b, w_out, b_out, out)
     return out

@@ -157,6 +157,7 @@ int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, const int32_
  *   residual_f32 / ls_gamma: the VGGT block form (vggt/layers/block.py:77-98 under autocast): the residual stream is
  *        float32, `residual` then points to float32 with Y's geometry (Y float32, may alias), and
  *        Y = residual + ls_gamma[n] * fp16(acc + bias)  with ls_gamma the float32 LayerScale vector (NULL = 1).
+ *        This form takes no gate: gate != NULL with residual_f32 is R3G_E_INVALID.
  *   qkn_*: the per-head q/k normalisation that follows a q/k/v projection, fused into the epilogue (the accumulator
  *        row of a 64-column head sits in one thread's registers): qkn_mode 1 = RMSNorm(64) with a learned scale
  *        (QKNorm, hunyuan3ddit.py:83-104,199,260), 2 = LayerNorm(64) with weight + bias (attention_blocks.py:315-316,
