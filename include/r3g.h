@@ -11,6 +11,16 @@
  *   - Return value: 0 = OK, negative = error (R3G_E_*); r3g_last_error(ctx) gives the message.
  *   - A context is bound to one device and is not thread-safe; distinct contexts are independent.
  *   - There is no CPU fallback: without a CUDA device every compute call returns R3G_E_CUDA.
+ *   - Programmatic dependent launch (PDL): r3g_linear, r3g_attention, r3g_layernorm, r3g_lnpost_dot, r3g_gemv,
+ *     r3g_swiglu, r3g_gemv_f32, r3g_layernorm_f32, r3g_small_attention_f32, r3g_im2col3x3 and r3g_bilinear_nhwc launch
+ *     their kernels with the programmatic-stream-serialization attribute, eagerly and under CUDA-graph capture, so a
+ *     kernel's prologue may run under the tail of the kernel before it in the stream.  Each waits (griddepcontrol.wait)
+ *     for that kernel to complete before it touches memory another kernel produces or still reads, with two
+ *     exceptions: r3g_layernorm reads w and b, and r3g_lnpost_dot reads ln_w, ln_b and w_out, before the wait.  The
+ *     launch immediately before either of them in the stream must therefore not write those buffers.  The r3g_linear
+ *     and r3g_attention prologues touch only kernel parameters and shared memory.  The environment variable R3G_PDL,
+ *     read once per context when it first launches such a kernel, controls this: unset or any value not starting with
+ *     '0' enables PDL, "0" launches every kernel in plain stream order.  Results are the same bits either way.
  */
 #ifndef R3G_H
 #define R3G_H
