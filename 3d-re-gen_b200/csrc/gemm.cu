@@ -5,7 +5,8 @@
 //   warps 0..7  two consumer warpgroups (wgmma.mma_async m64nBNk16, fp16 in, fp32 accumulators in registers; warpgroup
 //               g computes rows [64 g, 64 g + 64) of the tile).  After the main loop the accumulators are staged as an
 //               fp32 tile in the (then idle) operand ring and each of the 256 threads runs the epilogue for one row and
-//               half of the columns: bias, GELU, gate*y+residual, fp16/fp32 conversion, 16-byte global stores.
+//               half of the columns: bias, GELU, gate*y+residual, fp16/fp32 conversion, written back over its staged
+//               row; each warp then stores its 32 rows x BN/2 columns as coalesced 16-byte accesses.
 // Covers every nn.Linear on the hot path: DiT qkv/proj/mlp/linear1/linear2 (hunyuan3ddit.py:196-216,259-267),
 // ShapeVAE c_qkv/c_proj/c_fc (attention_blocks.py:166-182,345-363), geo-decoder query_proj/c_q/c_kv/c_proj/mlp
 // (attention_blocks.py:250-261,484-494).
@@ -128,9 +129,11 @@ __device__ __forceinline__ int stage_tile_operands(const LinearParams& p, uint4*
 // One 32-column chunk of one accumulator row: v = fp32 accumulators of columns [n0, n0+32) of logical row r.
 // sbias / sgate: this chunk's 4 uint4 of the staged slices (sgate NULL: gate from global memory or no gate);
 // `pre` holds this chunk's residual and is refilled for chunk next_n0 (>= 0) as soon as it has been consumed.
+// The result overwrites the chunk's own staged accumulators (fp16: the first 64 of its 128 bytes, fp32: all of them);
+// store_rows() moves it to global memory.
 __device__ __forceinline__ void epilogue_chunk(const LinearParams& p, const uint32_t* v, int r, int64_t out_row,
                                                int n0, const uint4* sbias, const uint4* sgate, const __half* gate_row,
-                                               ChunkOperands& pre, int next_n0) {
+                                               ChunkOperands& pre, int next_n0, uint4* sout) {
     float f[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
@@ -201,11 +204,11 @@ __device__ __forceinline__ void epilogue_chunk(const LinearParams& p, const uint
       }
     }
     if (p.out_f32) {
-      float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.y) + out_row * p.ldy + n0);
+      float4* op = reinterpret_cast<float4*>(sout);
 #pragma unroll
       for (int q = 0; q < 8; ++q) op[q] = make_float4(f[4 * q], f[4 * q + 1], f[4 * q + 2], f[4 * q + 3]);
     } else {
-      uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.y) + out_row * p.ldy + n0);
+      uint4* op = sout;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         uint4 o;
@@ -222,9 +225,10 @@ __device__ __forceinline__ void epilogue_chunk(const LinearParams& p, const uint
 // One 64-column head of one accumulator row with the q/k normalisation fused (qkn_mode): v0 / v1 = the two 32-column
 // accumulator chunks of columns [n0, n0+64).  Same arithmetic as qk_norm_kernel (rowops.cu): the Linear output is an
 // fp16 tensor, the statistics are fp32, RMS: (x * rrms).to(fp16) * scale; LayerNorm: (x - mean) * rstd * w + b.
+// The result overwrites the staged accumulators like epilogue_chunk's: each 32-column half at the start of its chunk
+// (sout: the first chunk's 128 bytes, the second's follow).
 __device__ __forceinline__ void epilogue_qknorm(const LinearParams& p, const uint32_t* v0, const uint32_t* v1,
-                                                int64_t out_row, int n0, const __half* nw, const __half* nb,
-                                                const uint4* sbias8) {
+                                                const __half* nw, const __half* nb, const uint4* sbias8, uint4* sout) {
   float f[64];
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
@@ -299,7 +303,6 @@ __device__ __forceinline__ void epilogue_qknorm(const LinearParams& p, const uin
       }
     }
   }
-  uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.y) + out_row * p.ldy + n0);
 #pragma unroll
   for (int q = 0; q < 8; ++q) {
     uint4 o;
@@ -307,7 +310,35 @@ __device__ __forceinline__ void epilogue_qknorm(const LinearParams& p, const uin
     o.y = pack_half2(f[8 * q + 2], f[8 * q + 3]);
     o.z = pack_half2(f[8 * q + 4], f[8 * q + 5]);
     o.w = pack_half2(f[8 * q + 6], f[8 * q + 7]);
-    op[q] = o;
+    sout[q + (q & 4)] = o;
+  }
+}
+
+// Global stores of one epilogue warp's region: the 32 rows of the tile starting at segment row l0 (rows at or past
+// seg_len are skipped), columns [n_start, n_start + ncols) (ncols <= 128, a multiple of 32).  srow0 points at the first
+// row's staged results: each 32-column chunk's fp16 output in the first 64 of its 128 bytes, fp32 output filling them.
+// A thread's epilogue owns a row, so a direct store would touch 32 rows per instruction; here 16 (fp16) or 32 (fp32)
+// lanes write 256 or 512 contiguous bytes of one row.
+template <int LD>
+__device__ __forceinline__ void store_rows(const LinearParams& p, const float* srow0, int lane, int l0, int sg,
+                                           int n_start, int ncols) {
+  __syncwarp();   // every lane's results are in shared memory
+  const int64_t row0 = (int64_t)sg * p.y_seg_stride + l0;
+  if (p.out_f32) {
+#pragma unroll 4
+    for (int i = 0; i < 32; ++i) {
+      if (l0 + i < p.seg_len && lane * 4 < ncols)
+        *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.y) + (row0 + i) * p.ldy + n_start + lane * 4) =
+            *reinterpret_cast<const float4*>(srow0 + i * LD + lane * 4);
+    }
+  } else {
+    const int j = lane & 15;   // 16-byte piece of the row: chunk j / 4, bytes 16 (j % 4) of its fp16 output
+#pragma unroll 4
+    for (int i = lane >> 4; i < 32; i += 2) {
+      if (l0 + i < p.seg_len && j * 8 < ncols)
+        *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.y) + (row0 + i) * p.ldy + n_start + j * 8) =
+            *reinterpret_cast<const uint4*>(srow0 + i * LD + 32 * (j >> 2) + 4 * (j & 3));
+    }
   }
 }
 
@@ -445,7 +476,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
   const int r = sg * p.seg_len + l;                          // logical row
   const int64_t out_row = (int64_t)sg * p.y_seg_stride + l;
   const __half* gate_row = p.gate ? p.gate + (int64_t)(row_ok ? r / p.gate_rows : 0) * p.gate_ld : nullptr;
-  const float* srow = acc_smem + row_in_tile * C::kLdStage;
+  float* srow = acc_smem + row_in_tile * C::kLdStage;
   ChunkOperands pre;
   bool have_pre = false;
 #pragma unroll 1
@@ -454,10 +485,11 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
     if (n0 >= p.N) break;  // warp-uniform
     const uint4* sbias = wsm + ((c0 - col_half * (BN / 2)) >> 3);
     const uint32_t* v = reinterpret_cast<const uint32_t*>(srow + c0);
+    uint4* sout = reinterpret_cast<uint4*>(srow + c0);
     const int nr = ((c0 & 32) == 0) ? qkn_range(p, n0) : -1;   // warp-uniform
     if (nr >= 0) {
       if (row_ok)
-        epilogue_qknorm(p, v, v + 32, out_row, n0, nr ? p.qkn_k_w : p.qkn_q_w, nr ? p.qkn_k_b : p.qkn_q_b, sbias);
+        epilogue_qknorm(p, v, v + 32, nr ? p.qkn_k_w : p.qkn_q_w, nr ? p.qkn_k_b : p.qkn_q_b, sbias, sout);
       c0 += 32;
       have_pre = false;
       continue;
@@ -468,9 +500,13 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
                       !((c1 & 32) == 0 && qkn_range(p, tn * BN + c1) >= 0);
     if (row_ok)
       epilogue_chunk(p, v, r, out_row, n0, sbias, gsel >= 0 ? sbias + 16 + 16 * gsel : nullptr, gate_row, pre,
-                     more ? tn * BN + c1 : -1);
+                     more ? tn * BN + c1 : -1, sout);
     have_pre = more;
   }
+  // the warp's 32 rows x (at most) BN / 2 columns, now in the staged rows, go out as coalesced 16-byte stores
+  const int n_start = tn * BN + col_half * (BN / 2);
+  store_rows<C::kLdStage>(p, acc_smem + (row_in_tile - lane) * C::kLdStage + col_half * (BN / 2), lane, l - lane, sg,
+                          n_start, min(BN / 2, p.N - n_start));
 }
 
 // One problem of a launch: tensor maps + kernel parameters.  tile_m = rows per tile, box_n = rows of W one CTA fetches
