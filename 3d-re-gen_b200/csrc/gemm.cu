@@ -612,11 +612,317 @@ int validate_linear(r3g_ctx* ctx, const r3g_linear_args* a) {
   return R3G_OK;
 }
 
+// ------------------------------------------------------------------------------------------ mixture of experts
+// (r3g_linear moe_mode; include/r3g.h).  MoEGate with N <= 64 experts is a GEMV-sized problem per row: one warp per row
+// computes the logits, the softmax, the top-k and the slot assignment, and copies the row into each chosen slot.
+constexpr int kRouteWarps = 8;
+constexpr int kMaxExperts = 64;
+
+__global__ void __launch_bounds__(32 * kRouteWarps)
+moe_route_kernel(const __half* __restrict__ x, int64_t ldx, const __half* __restrict__ wg, __half* __restrict__ logits,
+                 int64_t ldl, int M, int K, int E, int top_k, int cap, int32_t* __restrict__ counts,
+                 int32_t* __restrict__ ids, __half* __restrict__ weights, int32_t* __restrict__ slots,
+                 __half* __restrict__ slot_x, __half* __restrict__ slot_scale) {
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * kRouteWarps + (threadIdx.x >> 5);
+  if (r >= M) return;
+  const __half* xr = x + (int64_t)r * ldx;
+  // expert e's fp16 logit ends up in lane e % 32, register e / 32
+  float lg[2] = {-INFINITY, -INFINITY};
+  for (int e = 0; e < E; ++e) {
+    const __half* we = wg + (int64_t)e * K;
+    float acc = 0.f;
+    for (int k = lane * 8; k < K; k += 256) {
+      float a[8], b[8];
+      unpack8(*reinterpret_cast<const Half8*>(xr + k), a);
+      unpack8(*reinterpret_cast<const Half8*>(we + k), b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc = fmaf(a[j], b[j], acc);
+    }
+    acc = rnd_h(warp_sum(acc));
+    if (lane == (e & 31)) lg[e >> 5] = acc;
+  }
+  for (int h = 0; h < 2; ++h)
+    if (h * 32 + lane < E) logits[(int64_t)r * ldl + h * 32 + lane] = __float2half_rn(lg[h]);
+  // softmax over the fp16 logits in fp32, scores rounded to fp16 (torch's half softmax)
+  float mx = fmaxf(lg[0], lg[1]);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  float ex[2];
+  for (int h = 0; h < 2; ++h) ex[h] = h * 32 + lane < E ? expf(lg[h] - mx) : 0.f;
+  const float inv = 1.f / warp_sum(ex[0] + ex[1]);
+  float sc[2];
+  for (int h = 0; h < 2; ++h) sc[h] = h * 32 + lane < E ? rnd_h(ex[h] * inv) : -1.f;
+  for (int j = 0; j < top_k; ++j) {
+    // the highest score, equal scores to the lower expert index
+    float bv = sc[0] >= sc[1] ? sc[0] : sc[1];
+    int be = sc[0] >= sc[1] ? lane : 32 + lane;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oe = __shfl_xor_sync(0xffffffffu, be, o);
+      if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; }
+    }
+    if (lane == (be & 31)) sc[be >> 5] = -1.f;   // taken
+    int slot = 0;
+    if (lane == 0) {
+      slot = be * cap + atomicAdd(&counts[be], 1);
+      const int64_t o = (int64_t)r * top_k + j;
+      ids[o] = be;
+      weights[o] = __float2half_rn(bv);
+      slots[o] = slot;
+      slot_scale[slot] = __float2half_rn(bv);
+    }
+    slot = __shfl_sync(0xffffffffu, slot, 0);
+    __half* dst = slot_x + (int64_t)slot * K;
+    for (int k = lane * 8; k < K; k += 256) *reinterpret_cast<uint4*>(dst + k) = *reinterpret_cast<const uint4*>(xr + k);
+  }
+}
+
+// Grouped expert GEMM (moe_mode 2) and the shared expert's combine GEMM (moe_mode 3): linear_kernel<128>'s producer,
+// main loop and accumulator staging, so that a row's accumulators are those r3g_linear computes for it, with a per-row
+// epilogue in which each thread writes its own row.  No PDL: the row counts come from the route launch before it.
+struct MoeParams {
+  int M, N, K;               // M: rows per group (grouped) or rows (combine)
+  int groups, experts, tiles_m, tiles_n;
+  const int32_t* counts;
+  const __half* bias;        // [groups, N]
+  __half* y;
+  int64_t ldy;
+  int act;
+  const __half* row_scale;   // [groups * M]
+  const __half* residual;    // combine
+  const __half* slot_y;      // combine: [*, N]
+  const int32_t* slots;
+  const int32_t* ids;
+  int top_k;
+};
+
+__global__ void __launch_bounds__(kNumThreads, Cfg<128>::kMinBlocks)
+moe_gemm_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                const __grid_constant__ MoeParams p) {
+  using C = Cfg<128>;
+  constexpr int BN = 128;
+  const int per_group = p.tiles_m * p.tiles_n;
+  const int g = blockIdx.x / per_group, lt = blockIdx.x % per_group;
+  const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
+  const int rows = g < p.experts ? p.counts[g] : p.M;
+  if (tm * BM >= rows) return;   // surplus tile of the worst-case grid: the whole CTA leaves before any barrier
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
+  uint64_t* empty_bar = full_bar + C::kStages;
+  float* acc_smem = reinterpret_cast<float*>(smem);
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_k_blocks = (p.K + BK - 1) / BK;
+  const int row0 = g * p.M + tm * BM;   // first x / y row of the tile
+
+  if (warp == kNumEpilogueWarps && lane == 0) {
+    tma_prefetch_desc(&tmap_x);
+    tma_prefetch_desc(&tmap_w);
+    for (int s = 0; s < C::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 32 * kNumEpilogueWarps);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == kNumEpilogueWarps) {
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kb = 0; kb < num_k_blocks; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * C::kStageBytes;
+        mbar_expect_tx(&full_bar[stage], C::kStageBytes);
+        tma_load_2d(sa, &tmap_x, &full_bar[stage], kb * BK, row0, kEvictFirst);
+        tma_load_2d(sa + C::kStageBytesA, &tmap_w, &full_bar[stage], kb * BK, g * p.N + tn * BN, kEvictLast);
+        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+      }
+    }
+    return;
+  }
+
+  const int wg = warp >> 2;
+  {
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * C::kStageBytes) + wg * 64 * 128;
+      const uint32_t sb = smem_u32(smem + stage * C::kStageBytes + C::kStageBytesA);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        wgmma_tile<BN>(acc, gmma_desc_sw128(sa + k * 32, 1024, 16), gmma_desc_sw128(sb + k * 32, 1024, 16));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (kb > 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence<BN / 2>(acc);
+    named_bar_sync(1, 32 * kNumEpilogueWarps);
+    const int w4 = warp & 3;
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = wg * 64 + w4 * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+      const int col = 8 * (i >> 2) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(acc_smem + row * C::kLdStage + col) = make_float2(acc[i], acc[i + 1]);
+    }
+    named_bar_sync(1, 32 * kNumEpilogueWarps);
+  }
+
+  // epilogue: one row, half of the tile's columns, 8 columns at a time
+  const int row_in_tile = threadIdx.x & (BM - 1);
+  const int col_half = threadIdx.x >> 7;
+  if (tm * BM + row_in_tile >= rows) return;
+  const int64_t yr = row0 + row_in_tile;
+  const float* srow = acc_smem + row_in_tile * C::kLdStage;
+  const float scale = p.row_scale ? __half2float(p.row_scale[yr]) : 1.f;
+  int64_t src[4] = {0, 0, 0, 0};   // combine: the row's slots in increasing expert order
+  if (p.slot_y) {
+    int e[4];
+    for (int j = 0; j < p.top_k; ++j) { e[j] = p.ids[yr * p.top_k + j]; src[j] = p.slots[yr * p.top_k + j]; }
+    for (int i = 1; i < p.top_k; ++i)
+      for (int j = i; j > 0 && e[j - 1] > e[j]; --j) {
+        const int te = e[j]; e[j] = e[j - 1]; e[j - 1] = te;
+        const int64_t ts = src[j]; src[j] = src[j - 1]; src[j - 1] = ts;
+      }
+  }
+#pragma unroll 1
+  for (int c = col_half * (BN / 2); c < (col_half + 1) * (BN / 2); c += 8) {
+    const int n = tn * BN + c;
+    if (n >= p.N) break;
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] = srow[c + j];
+    if (p.bias) {
+      float b[8];
+      unpack8(*reinterpret_cast<const Half8*>(p.bias + (int64_t)g * p.N + n), b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] += b[j];
+    }
+    if (p.act == 2) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = gelu_erf_f(rnd_h(f[j]));
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] = rnd_h(f[j]);
+    if (p.row_scale) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = rnd_h(f[j] * scale);
+    }
+    if (p.slot_y) {
+      float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, t[8], res[8];
+      for (int k = 0; k < p.top_k; ++k) {
+        unpack8(*reinterpret_cast<const Half8*>(p.slot_y + src[k] * p.N + n), t);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s[j] = rnd_h(s[j] + t[j]);
+      }
+      unpack8(*reinterpret_cast<const Half8*>(p.residual + yr * p.ldy + n), res);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = res[j] + rnd_h(s[j] + f[j]);
+    }
+    *reinterpret_cast<Half8*>(p.y + yr * p.ldy + n) = pack8(f);
+  }
+}
+
+int launch_moe_route(r3g_ctx* ctx, const r3g_linear_args* a, cudaStream_t s) {
+  const int E = a->moe_experts;
+  if (a->N != E || E < 1 || E > kMaxExperts || a->moe_top_k < 1 || a->moe_top_k > 4 || a->moe_top_k > E ||
+      a->moe_cap < a->M || a->K % 8 || a->ldx % 8 || a->bias || !a->moe_counts || !a->moe_ids || !a->moe_weights ||
+      !a->moe_slots || !a->moe_slot_x || !a->moe_slot_scale)
+    return r3g_fail(ctx, R3G_E_INVALID, "linear (moe route): need N == moe_experts <= %d, 1 <= moe_top_k <= min(4, N), "
+                    "moe_cap >= M, K %% 8 == 0, no bias and every moe buffer (N=%d experts=%d top_k=%d)", kMaxExperts,
+                    a->N, E, a->moe_top_k);
+  R3G_CUDA_OK(ctx, cudaMemsetAsync(a->moe_counts, 0, sizeof(int32_t) * E, s));
+  moe_route_kernel<<<(a->M + kRouteWarps - 1) / kRouteWarps, 32 * kRouteWarps, 0, s>>>(
+      (const __half*)a->x, a->ldx, (const __half*)a->w, (__half*)a->y, a->ldy, a->M, a->K, E, a->moe_top_k, a->moe_cap,
+      a->moe_counts, a->moe_ids, (__half*)a->moe_weights, a->moe_slots, (__half*)a->moe_slot_x,
+      (__half*)a->moe_slot_scale);
+  R3G_LAUNCH_OK(ctx);
+  return R3G_OK;
+}
+
+int launch_moe_gemm(r3g_ctx* ctx, const r3g_linear_args* a, cudaStream_t s) {
+  const bool combine = a->moe_mode == R3G_MOE_COMBINE;
+  const int groups = combine ? 1 : a->moe_groups;
+  if (a->N % 8 || a->K % 8 || a->ldx % 8 || a->ldy % 8 || groups < 1)
+    return r3g_fail(ctx, R3G_E_INVALID, "linear (moe): need N %% 8 == 0, K %% 8 == 0, ldx/ldy %% 8 == 0, moe_groups >= 1");
+  if ((a->act != 0 && a->act != 2) || (combine && a->act))
+    return r3g_fail(ctx, R3G_E_INVALID, "linear (moe): act must be 0, or 2 (erf-GELU) in grouped mode");
+  if (combine ? (!a->residual || !a->moe_slot_y || !a->moe_slots || !a->moe_ids || a->moe_top_k < 1 ||
+                 a->moe_top_k > 4 || a->moe_slot_scale)
+              : (a->moe_experts < 0 || a->moe_experts > groups || a->moe_cap != a->M ||
+                 (a->moe_experts && !a->moe_counts) || a->residual || a->moe_slot_y))
+    return r3g_fail(ctx, R3G_E_INVALID, "linear (moe %s): inconsistent moe operands", combine ? "combine" : "grouped");
+  Problem pr;
+  memset(&pr, 0, sizeof(pr));
+  {
+    const uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)groups * a->M};
+    const uint64_t strides[2] = {2, (uint64_t)a->ldx * 2};
+    const uint32_t box[2] = {BK, BM};
+    int rc = r3g_make_tmap_f16(ctx, &pr.tx, a->x, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  {
+    const uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)groups * a->N};
+    const uint64_t strides[2] = {2, (uint64_t)a->K * 2};
+    const uint32_t box[2] = {BK, 128};
+    int rc = r3g_make_tmap_f16(ctx, &pr.tw, a->w, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  MoeParams p;
+  memset(&p, 0, sizeof(p));
+  p.M = a->M; p.N = a->N; p.K = a->K;
+  p.groups = groups;
+  p.experts = combine ? 0 : a->moe_experts;
+  p.tiles_m = (a->M + BM - 1) / BM;
+  p.tiles_n = (a->N + 127) / 128;
+  p.counts = a->moe_counts;
+  p.bias = (const __half*)a->bias;
+  p.y = (__half*)a->y; p.ldy = a->ldy;
+  p.act = a->act;
+  p.row_scale = (const __half*)a->moe_slot_scale;
+  if (combine) {
+    p.residual = (const __half*)a->residual;
+    p.slot_y = (const __half*)a->moe_slot_y;
+    p.slots = a->moe_slots;
+    p.ids = a->moe_ids;
+    p.top_k = a->moe_top_k;
+  }
+  using C = Cfg<128>;
+  if (!(ctx->attr_done & R3G_ATTR_MOE_GEMM)) {
+    R3G_CUDA_OK(ctx, cudaFuncSetAttribute(moe_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
+    ctx->attr_done |= R3G_ATTR_MOE_GEMM;
+  }
+  moe_gemm_kernel<<<(unsigned)(groups * p.tiles_m * p.tiles_n), kNumThreads, C::kSmemBytes, s>>>(pr.tx, pr.tw, p);
+  R3G_LAUNCH_OK(ctx);
+  return R3G_OK;
+}
+
 }  // namespace
 
 extern "C" int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream) {
   R3G_ENTRY(ctx, "linear");
   if (!a) return r3g_fail(ctx, R3G_E_INVALID, "linear: null argument");
+  if (a->moe_mode) {
+    if (a->moe_mode < R3G_MOE_ROUTE || a->moe_mode > R3G_MOE_COMBINE)
+      return r3g_fail(ctx, R3G_E_INVALID, "linear: unknown moe_mode %d", a->moe_mode);
+    if (!a->x || !a->w || !a->y || a->group_next || a->gate || a->out_f32 || a->residual_f32 || a->ls_gamma ||
+        a->qkn_mode || a->seg_len || (a->moe_mode == R3G_MOE_ROUTE && a->act))
+      return r3g_fail(ctx, R3G_E_INVALID, "linear (moe): no group_next, gate, fp32, qkn or segment operands");
+    if (a->M <= 0) return R3G_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    return a->moe_mode == R3G_MOE_ROUTE ? launch_moe_route(ctx, a, s) : launch_moe_gemm(ctx, a, s);
+  }
   // the non-empty problems of the group_next chain, in order
   const r3g_linear_args* probs[kMaxGroup];
   int n = 0, len = 0;

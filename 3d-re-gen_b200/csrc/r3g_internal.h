@@ -26,7 +26,7 @@ struct r3g_ctx {
   int pdl;                     // -1 = environment not read yet; R3G_PDL=0 disables programmatic dependent launch
 };
 enum { R3G_ATTR_ATTENTION = 1, R3G_ATTR_LINEAR128 = 4, R3G_ATTR_LINEAR256 = 8,
-       R3G_ATTR_MISC0 = 32, R3G_ATTR_MISC1 = 64, R3G_ATTR_MISC2 = 128 };
+       R3G_ATTR_MISC0 = 32, R3G_ATTR_MISC1 = 64, R3G_ATTR_MISC2 = 128, R3G_ATTR_MOE_GEMM = 256 };
 
 // Every ABI entry point runs with the context's device current (a kernel cannot be launched into a stream of
 // another device) and restores the caller's device on return.

@@ -164,17 +164,23 @@ __device__ __forceinline__ float head_sum(float s) {   // over the 8 lanes of a 
 // Normalises in place the 8 features f this lane (sub = lane & 7) holds of a 64-wide head:
 //   rms:  f = fp16(f * rrms) * w            ((x*rrms).to(fp16) * scale)
 //   else: f = (f - mean) * rstd * w + b     (LayerNorm, b optional)
-__device__ __forceinline__ void norm_head8(float (&f)[8], bool rms, float eps, const __half* w, const __half* b,
+//   mode 2 (torch's nn.RMSNorm, one rounding): f = f * rrms * w
+__device__ __forceinline__ void norm_head8(float (&f)[8], int mode, float eps, const __half* w, const __half* b,
                                            int sub) {
   float wf[8];
   unpack8(reinterpret_cast<const Half8*>(w)[sub], wf);
-  if (rms) {
+  if (mode != 1) {
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) s += f[i] * f[i];
     const float rrms = rsqrtf(head_sum(s) * (1.f / 64.f) + eps);
+    if (mode == 0) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) f[i] = rnd_h(f[i] * rrms) * wf[i];
+      for (int i = 0; i < 8; ++i) f[i] = rnd_h(f[i] * rrms) * wf[i];
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) f[i] = f[i] * rrms * wf[i];
+    }
     return;
   }
   float s = 0.f;
@@ -212,7 +218,7 @@ __global__ void __launch_bounds__(256) qk_norm_kernel(__half* __restrict__ buf, 
   __half* p = buf + row * ld + (sel ? k_off : q_off) + (int64_t)h * head_stride + sub * 8;
   float f[8];
   unpack8(*reinterpret_cast<const Half8*>(p), f);
-  norm_head8(f, mode == 0, eps, sel ? k_w : q_w, sel ? k_b : q_b, sub);
+  norm_head8(f, mode, eps, sel ? k_w : q_w, sel ? k_b : q_b, sub);
   if (active) *reinterpret_cast<Half8*>(p) = pack8(f);
 }
 
@@ -294,7 +300,7 @@ __global__ void __launch_bounds__(256) qk_norm_rope_kernel(__half* __restrict__ 
   float f[8];
   unpack8(*reinterpret_cast<const Half8*>(p), f);
   const __half* wv = sel ? k_w : q_w;
-  if (wv) norm_head8(f, false, eps, wv, sel ? k_b : q_b, sub);
+  if (wv) norm_head8(f, 1, eps, wv, sel ? k_b : q_b, sub);
   float partner[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) partner[i] = __shfl_xor_sync(0xffffffffu, f[i], 2);
@@ -771,6 +777,7 @@ extern "C" int r3g_qk_norm(r3g_ctx* ctx, void* buf, int64_t ld, int rows, int he
   R3G_ENTRY(ctx, "qk_norm");
   if (ld % 8 || q_off % 8 || k_off % 8 || head_stride % 8 || !q_w)
     return r3g_fail(ctx, R3G_E_INVALID, "qk_norm: offsets/strides must be multiples of 8 halfs");
+  if (mode < 0 || mode > 2) return r3g_fail(ctx, R3G_E_INVALID, "qk_norm: mode must be 0, 1 or 2, got %d", mode);
   if (!r3g_aligned16(buf) || !r3g_aligned16(q_w) || !r3g_aligned16(q_b) || !r3g_aligned16(k_w) || !r3g_aligned16(k_b))
     return r3g_fail(ctx, R3G_E_INVALID, "qk_norm: pointers must be 16-byte aligned");
   const int nsel = k_w ? 2 : 1;

@@ -34,6 +34,10 @@ class LinearArgs(C.Structure):
         ("qkn_eps", C.c_float),
         ("qkn_q_w", C.c_void_p), ("qkn_q_b", C.c_void_p), ("qkn_k_w", C.c_void_p), ("qkn_k_b", C.c_void_p),
         ("group_next", C.c_void_p),
+        ("moe_mode", C.c_int), ("moe_groups", C.c_int), ("moe_experts", C.c_int), ("moe_top_k", C.c_int),
+        ("moe_cap", C.c_int),
+        ("moe_counts", C.c_void_p), ("moe_ids", C.c_void_p), ("moe_weights", C.c_void_p), ("moe_slots", C.c_void_p),
+        ("moe_slot_x", C.c_void_p), ("moe_slot_scale", C.c_void_p), ("moe_slot_y", C.c_void_p),
     ]
 
 

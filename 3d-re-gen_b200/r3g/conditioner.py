@@ -17,6 +17,11 @@ from . import ops
 DINOV2_GIANT = dict(hidden_size=1536, num_hidden_layers=40, num_attention_heads=24, mlp_ratio=4, patch_size=14,
                     image_size=518, use_swiglu_ffn=True, layerscale_value=1.0, qkv_bias=True,
                     hidden_act="gelu", layer_norm_eps=1e-6)
+# DINOv2-large (Hunyuan3D-2mini's conditioner, UNVERIFIED: its config.yaml is not in the reference tree): a GELU MLP,
+# so DinoImageEncoder picks the HF backend for it
+DINOV2_LARGE = dict(hidden_size=1024, num_hidden_layers=24, num_attention_heads=16, mlp_ratio=4, patch_size=14,
+                    image_size=518, use_swiglu_ffn=False, layerscale_value=1.0, qkv_bias=True,
+                    hidden_act="gelu", layer_norm_eps=1e-6)
 
 
 class DinoImageEncoder:

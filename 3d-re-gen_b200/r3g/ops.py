@@ -195,6 +195,76 @@ def linear_pair(first, second):
     return linear_group(first, second)
 
 
+MOE_ROUTE, MOE_GROUPED, MOE_COMBINE = 1, 2, 3
+
+
+def _moe_buf(t, dev, name, dtype, numel):
+    """A contiguous `dtype` buffer of at least `numel` elements on cuda:dev, as its address."""
+    if t.dtype != dtype or not t.is_contiguous() or t.numel() < numel:
+        raise ValueError(f"moe: {name} must be a contiguous {dtype} buffer of at least {numel} elements, got "
+                         f"{t.dtype} {tuple(t.shape)}")
+    return _ptr(t, dev, "linear", name)
+
+
+def moe_route(x, w, *, top_k, cap, slot_x, slot_scale, counts, ids, weights, slots, out=None):
+    """MoEGate.forward and the dispatch of its rows (r3g_linear moe_mode 1, include/r3g.h).  x: [M, K] rows, w: the gate
+    weight [E, K] (E <= 64); out: fp16 [M, E] logits.  Writes ids / slots int32 [M, top_k], weights fp16 [M, top_k],
+    counts int32 [E], and each chosen (row, expert) copy of x into slot_x [E * cap, K] with its weight in slot_scale."""
+    dev = x.get_device()
+    a, out = _linear_args(dev, x, w, out=out)
+    E, K, M = w.shape[0], w.shape[1], a.M
+    a.moe_mode, a.moe_experts, a.moe_top_k, a.moe_cap = MOE_ROUTE, E, top_k, cap
+    a.moe_counts = _moe_buf(counts, dev, "counts", torch.int32, E)
+    a.moe_ids = _moe_buf(ids, dev, "ids", torch.int32, M * top_k)
+    a.moe_weights = _moe_buf(weights, dev, "weights", torch.float16, M * top_k)
+    a.moe_slots = _moe_buf(slots, dev, "slots", torch.int32, M * top_k)
+    a.moe_slot_x = _moe_buf(slot_x, dev, "slot_x", torch.float16, E * cap * K)
+    a.moe_slot_scale = _moe_buf(slot_scale, dev, "slot_scale", torch.float16, E * cap)
+    _launch("linear", x, C.byref(a))
+    return out
+
+
+def moe_grouped(x, w, bias=None, *, counts, experts, out, act=ACT_NONE, row_scale=None):
+    """G = w.shape[0] GEMMs in one launch (r3g_linear moe_mode 2): x [G * cap, K] holds one cap-row segment per group,
+    w [G, N, K], bias [G, N]; group g < experts has counts[g] rows (read on the device), the others cap; out [G * cap,
+    N] receives fp16(act(x w[g]^T + bias[g])), times row_scale[row] (fp16 [G * cap]) after the rounding if given."""
+    G, N, K = w.shape
+    if x.dim() != 2 or x.shape[0] % G or not w.is_contiguous():
+        raise ValueError("moe_grouped: x must be [G * cap, K] and w a contiguous [G, N, K]")
+    dev = x.get_device()
+    if bias is not None and (tuple(bias.shape) != (G, N) or not bias.is_contiguous()):
+        raise ValueError(f"moe_grouped: bias must be a contiguous [{G}, {N}]")
+    cap = x.shape[0] // G
+    if out is None or tuple(out.shape) != (G * cap, N):
+        raise ValueError(f"moe_grouped: out must be [{G * cap}, {N}]")
+    # group 0's operands describe the launch; the kernel addresses group g at g times their sizes
+    a, _ = _linear_args(dev, x[:cap], w[0], None if bias is None else bias[0], out=out[:cap], act=act)
+    a.moe_mode, a.moe_groups, a.moe_experts, a.moe_cap = MOE_GROUPED, G, experts, cap
+    if experts:
+        a.moe_counts = _moe_buf(counts, dev, "counts", torch.int32, experts)
+    if row_scale is not None:
+        a.moe_slot_scale = _moe_buf(row_scale, dev, "row_scale", torch.float16, G * cap)
+    _launch("linear", x, C.byref(a))
+    return out
+
+
+def moe_combine(x, w, bias, *, slot_y, ids, slots, residual, out):
+    """The shared expert's second Linear with the MoE sum and the block residual fused (r3g_linear moe_mode 3):
+    out = fp16(residual + fp16(routed + fp16(x w^T + bias))), routed = the fp16 sum, in increasing expert order, of the
+    rows slots[r] of slot_y (the weighted expert outputs)."""
+    dev = x.get_device()
+    a, out = _linear_args(dev, x, w, bias, out=out, residual=residual)
+    top_k = ids.shape[-1]
+    a.moe_mode, a.moe_top_k = MOE_COMBINE, top_k
+    a.moe_ids = _moe_buf(ids, dev, "ids", torch.int32, a.M * top_k)
+    a.moe_slots = _moe_buf(slots, dev, "slots", torch.int32, a.M * top_k)
+    if slot_y.shape[-1] != a.N or not slot_y.is_contiguous() or slot_y.dtype != torch.float16:
+        raise ValueError(f"moe_combine: slot_y must be a contiguous fp16 [*, {a.N}]")
+    a.moe_slot_y = _ptr(slot_y, dev, "linear", "slot_y")
+    _launch("linear", x, C.byref(a))
+    return out
+
+
 def attention(q, k, v, out=None, scale=None, windows=None):
     """softmax(q k^T * scale) v.  q: [B, Lq, H, 64] views (any strides with unit inner stride), k/v: [B, Lk, H, 64].
     Returns/writes out: [B, Lq, H, 64] ("B L (H D)" when contiguous).
@@ -280,7 +350,8 @@ def patchify(images, patch, mean=None, std=None, out_ld=None):
 
 
 def qk_norm_(buf, heads, q_off, k_off, head_stride, mode, eps, q_w, q_b=None, k_w=None, k_b=None):
-    """In-place per-head RMS (mode 0) / LayerNorm (mode 1) of q (and k) inside a packed buffer of rows
+    """In-place per-head RMS (mode 0: QKNorm, rounded before the scale) / LayerNorm (mode 1) / nn.RMSNorm (mode 2: one
+    rounding) of q (and k) inside a packed buffer of rows
     ([rows, ld] or a segmented [S, L, ld] view)."""
     _f16(buf, "buf")
     rows, _, ld, sl, sst = _rows(buf, "buf")

@@ -23,8 +23,9 @@ import torch
 
 from . import dist as r3g_dist
 from . import ops
-from .conditioner import SingleImageEncoder, image_encoder_class
+from .conditioner import DINOV2_LARGE, SingleImageEncoder, image_encoder_class
 from .dit import Hunyuan3DDiT
+from .dit_plain import HunYuanDiTPlain
 from .graphs import GraphCache
 from .preprocessors import ImageProcessorV2, MVImageProcessorV2
 from .scheduler import ConsistencyFlowMatchEulerDiscreteScheduler, FlowMatchEulerDiscreteScheduler
@@ -70,6 +71,42 @@ HUNYUAN3D_2MV_TURBO_CONFIG = dict(
     conditioner=HUNYUAN3D_2MV_CONFIG["conditioner"],
     image_processor=HUNYUAN3D_2MV_CONFIG["image_processor"],
 )
+
+# Hunyuan3D-2mini (`hunyuan3d-dit-v2-mini`, 0.6 B parameters; the default of src/2d_to_3d_models/run.py:148,154): the
+# HunYuanDiTPlain denoiser with a mixture-of-experts FFN in its last blocks, a 512-latent VAE and a DINOv2-large
+# conditioner.  UNVERIFIED: the checkpoint's config.yaml is downloaded at run time and is not in the reference tree;
+# every value below is an assumption, and every one is a constructor parameter.
+HUNYUAN3D_2MINI_CONFIG = dict(
+    model=dict(target="hy3dgen.shapegen.models.denoisers.hunyuandit.HunYuanDiTPlain", input_size=512, in_channels=64,
+               hidden_size=1024, context_dim=1024, depth=16, num_heads=16, qk_norm=True, qk_norm_type="rms",
+               text_len=1370, with_decoupled_ca=False, use_attention_pooling=False, qkv_bias=False,
+               num_moe_layers=6, num_experts=8, moe_top_k=2),
+    vae=dict(HUNYUAN3D_2_CONFIG["vae"], num_latents=512),
+    scheduler=dict(num_train_timesteps=1000),
+    conditioner=dict(type="DinoImageEncoder", kwargs=dict(config=DINOV2_LARGE, image_size=518, use_cls_token=True)),
+    image_processor=dict(size=512, border_ratio=0.15),
+)
+
+# `hunyuan3d-dit-v2-mini-turbo`: HunYuanDiTPlain has no guidance embedding, so the turbo checkpoint is the same
+# architecture run with CFG and the consistency scheduler (pcm_timesteps = 100 UNVERIFIED, as for 2.0-turbo)
+HUNYUAN3D_2MINI_TURBO_CONFIG = dict(HUNYUAN3D_2MINI_CONFIG, scheduler=HUNYUAN3D_2_TURBO_CONFIG["scheduler"])
+
+
+def denoiser_class(target):
+    """The denoiser a config's `model.target` names (pipelines.py:121-128 instantiates it).  None: Hunyuan3DDiT, the
+    2.0 / 2mv denoiser."""
+    if target is None or str(target).endswith(".Hunyuan3DDiT"):
+        return Hunyuan3DDiT
+    if str(target).endswith(".HunYuanDiTPlain"):
+        return HunYuanDiTPlain
+    raise NotImplementedError(f"model target {target!r}: only Hunyuan3DDiT and HunYuanDiTPlain (the Hunyuan3D-2 / "
+                              "-2mv / -2mini shape checkpoints') are mirrored")
+
+
+def _context_kv(model):
+    """A denoiser whose cross-attention k / v of the (step-invariant) context can be projected once per call
+    (HunYuanDiTPlain.project_context): that method, else None."""
+    return getattr(model, "project_context", None)
 
 
 def _guidance_distilled(model):
@@ -197,7 +234,8 @@ class Hunyuan3DDiTPipeline:
         config's `conditioner` type: DinoImageEncoder when it has none) or None (callers then pass precomputed `cond=`
         tensors).  The config's `image_processor.target` picks the image processor (image_processor_class)."""
         cfg = config or HUNYUAN3D_2_CONFIG
-        model = Hunyuan3DDiT(device=device, **cfg["model"]).init_random(seed)
+        mc = dict(cfg["model"])
+        model = denoiser_class(mc.pop("target", None))(device=device, **mc).init_random(seed)
         vae = ShapeVAE(device=device, **cfg["vae"]).init_random(seed + 1)
         sc = dict(cfg["scheduler"])
         sched = scheduler_class(sc.pop("target", None))(**sc)
@@ -234,7 +272,7 @@ class Hunyuan3DDiTPipeline:
                 ckpt.setdefault(name, {})[rest] = v
         else:
             ckpt = torch.load(ckpt_path, map_location="cpu", weights_only=True)
-        model = Hunyuan3DDiT(device=device, **config["model"]["params"])
+        model = denoiser_class(config["model"].get("target"))(device=device, **config["model"]["params"])
         model.load_state_dict(ckpt["model"])
         vae = ShapeVAE(device=device, **config["vae"]["params"])
         vae.load_state_dict(ckpt["vae"])
@@ -417,18 +455,28 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         if do_cfg and B == 1:
             un = ctx["main"][1]
             shared = bool(torch.equal(un, un[:1].expand_as(un)))
+        # the context's cross-attention k / v, once per call, outside the step graph (into a buffer the graph owns)
+        proj = _context_kv(self.model)
+        kv = proj(ctx["main"]) if proj is not None else None
         g = None
         if self.use_cuda_graph and self.model.taps is None:
-            g = self._graphs.get((x_in.shape, ctx["main"].shape, shared),
-                                 (x_in, t_buf, ctx["main"]) + ((guidance,) if guidance is not None else ()),
-                                 lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs}, uncond_txt_shared=shared,
-                                                                        **gkw(gs)))
+            if kv is not None:
+                g = self._graphs.get((x_in.shape, ctx["main"].shape, shared), (x_in, t_buf, ctx["main"], kv),
+                                     lambda xs, ts, cs, kvs: self.model(xs, ts, {"main": cs}, context_kv=kvs))
+                kv = proj(ctx["main"], out=g.inputs[3])
+            else:
+                g = self._graphs.get((x_in.shape, ctx["main"].shape, shared),
+                                     (x_in, t_buf, ctx["main"]) + ((guidance,) if guidance is not None else ()),
+                                     lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs},
+                                                                            uncond_txt_shared=shared, **gkw(gs)))
             g.inputs[0].copy_(x_in)
             g.inputs[2].copy_(ctx["main"])
             if guidance is not None:
                 g.inputs[3].copy_(guidance)
                 guidance = g.inputs[3]
             x_in, t_buf = g.inputs[:2]
+        if kv is not None:
+            gkw = lambda gs: {"context_kv": kv}  # noqa: E731
         for i in range(n):
             t_buf.copy_(t16[i].expand(x_in.shape[0]))
             if g is not None:
@@ -479,18 +527,27 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
             gkw = lambda gs: {} if gs is None else {"guidance": gs}  # noqa: E731
             t_buf = torch.full((1,), 0.5, device=self.device, dtype=torch.float16)
             x_in = x
+            proj = _context_kv(self.model)
+            kv = proj(ctx) if proj is not None else None
             g = None
             if self.use_cuda_graph and self.model.taps is None:
-                g = self._graphs.get((x.shape, ctx.shape, shared),
-                                     (x, t_buf, ctx) + ((guidance,) if guidance is not None else ()),
-                                     lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs},
-                                                                            uncond_txt_shared=shared, **gkw(gs)))
+                if kv is not None:
+                    g = self._graphs.get((x.shape, ctx.shape, shared), (x, t_buf, ctx, kv),
+                                         lambda xs, ts, cs, kvs: self.model(xs, ts, {"main": cs}, context_kv=kvs))
+                    kv = proj(ctx, out=g.inputs[3])
+                else:
+                    g = self._graphs.get((x.shape, ctx.shape, shared),
+                                         (x, t_buf, ctx) + ((guidance,) if guidance is not None else ()),
+                                         lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs},
+                                                                                uncond_txt_shared=shared, **gkw(gs)))
                 x_in, t_buf = g.inputs[:2]
                 x_in.copy_(x)
                 g.inputs[2].copy_(ctx)
                 if guidance is not None:
                     g.inputs[3].copy_(guidance)
                     guidance = g.inputs[3]
+            if kv is not None:
+                gkw = lambda gs: {"context_kv": kv}  # noqa: E731
             x = x_in            # the Euler update below rewrites the model input in place: no copy per step
             v_pair = torch.empty((2,) + tuple(x.shape[1:]), device=self.device, dtype=x.dtype) if do_cfg else None
             for i in range(n):

@@ -182,7 +182,32 @@ int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, const int32_
  *        of 3.  With the unconditional text collapsed to one row (r3g_attention windows) the txt stream is two
  *        problems, batch 0's 1370 rows and batch 1's single row: img + both fill 240 of the 264 tiles of 2 waves.
  *        Results are those of separate calls.
+ *   moe_*: the mixture-of-experts FFN of HunYuanDiTPlain's last blocks (moe_layers.py:50-151) without a host sync, in
+ *        three modes.  moe_mode 0 ignores every moe_* field.  Slot buffers hold one fixed-capacity segment of
+ *        moe_cap rows per group: group g's rows are rows [g * moe_cap, g * moe_cap + count_g).  A mode-1 or mode-3 call
+ *        takes no group_next, activation, gate, qkn or fp32 operands; its launches are plain stream-ordered (no PDL).
+ *     1 route (MoEGate.forward, :50-68): x [M, K] the LayerNorm rows, w [N, K] the gate weight with N = moe_experts
+ *        <= 64, y fp16 [M, N] receives the logits fp16(x . w^T) (bias must be NULL).  Per row, scores =
+ *        fp16(softmax(logits)) in fp32, then the moe_top_k highest scores (equal scores: lower expert first; the weights
+ *        are not renormalised).  For each of them, in decreasing score order j: moe_ids[r * top_k + j] = e,
+ *        moe_weights[...] = the fp16 score, a position p in e's segment (from an atomic counter: the order of rows
+ *        inside a segment varies between runs), moe_slots[...] = e * moe_cap + p, moe_slot_scale[e * moe_cap + p] =
+ *        the score, and x's row is copied to row e * moe_cap + p of moe_slot_x (fp16, K columns, leading dimension
+ *        K).  moe_counts (int32 [moe_experts]) is zeroed by the call and ends holding each expert's row count.
+ *        moe_cap >= M (an expert takes a row at most once).
+ *     2 grouped: moe_groups independent GEMMs in one launch, group g = x rows [g * moe_cap, ...) (ldx) against
+ *        w[g] (w is [moe_groups, N, K]) plus bias[g] (bias [moe_groups, N] or NULL), written to the same rows of y
+ *        (ldy), with act 0 or 2 (erf-GELU) over all columns.  Groups g < moe_experts have moe_counts[g] rows, read on
+ *        the device; the others have M rows (the shared expert's identity rows); M = moe_cap.  The grid covers moe_cap
+ *        rows of every group and the CTAs past a group's count exit.  moe_slot_scale (fp16 [moe_groups * moe_cap] or
+ *        NULL) scales each row after the fp16 rounding: y = fp16(fp16(acc + bias) * scale[row]).
+ *     3 combine: y = fp16(residual + fp16(fp16(routed) + fp16(acc + bias))) over M rows, where routed is the fp16
+ *        sum, from 0 in increasing expert order, of rows moe_slots[r * top_k + j] of moe_slot_y (fp16 [*, N],
+ *        leading dimension N), the weighted expert outputs of mode 2 (expert_cache + shared_experts(identity), then
+ *        the block's residual, moe_layers.py:105-106, hunyuandit.py:351-352).  residual (ldy) may alias y.
+ *        Every row's result is independent of the segment positions route chose, so repeated runs agree bit for bit.
  */
+enum { R3G_MOE_ROUTE = 1, R3G_MOE_GROUPED = 2, R3G_MOE_COMBINE = 3 };
 typedef struct {
   const void* x; int64_t ldx;
   const void* w;
@@ -200,6 +225,14 @@ typedef struct {
   float qkn_eps;
   const void* qkn_q_w; const void* qkn_q_b; const void* qkn_k_w; const void* qkn_k_b;
   const void* group_next;    /* NULL, or a second r3g_linear_args executed by the SAME launch */
+  int moe_mode, moe_groups, moe_experts, moe_top_k, moe_cap;
+  int32_t* moe_counts;       /* int32 [moe_experts] */
+  int32_t* moe_ids;          /* int32 [M, moe_top_k] */
+  void* moe_weights;         /* fp16 [M, moe_top_k] */
+  int32_t* moe_slots;        /* int32 [M, moe_top_k] */
+  void* moe_slot_x;          /* fp16 [moe_experts * moe_cap, K] */
+  void* moe_slot_scale;      /* fp16 [moe_groups * moe_cap] */
+  const void* moe_slot_y;    /* fp16 [moe_experts * moe_cap, N] */
 } r3g_linear_args;
 int r3g_linear(r3g_ctx* ctx, const r3g_linear_args* a, void* stream);
 
@@ -258,7 +291,9 @@ int r3g_patchify(r3g_ctx* ctx, const float* images, void* out, int64_t out_ld, i
  * Element (r, h, d) of q lives at buf + r*ld + q_off + h*head_stride + d (same for k with k_off).
  * mode 0: RMSNorm over d with learned scale, computed in fp32, rounded to fp16, THEN multiplied by the fp16
  *         scale (hunyuan3ddit.py:83-104).  mode 1: LayerNorm(eps) with weight and bias (attention_blocks.py:315-316,
- *         vggt/layers/attention.py:44-45).  k_w == NULL skips k (geo-decoder query side). */
+ *         vggt/layers/attention.py:44-45).  mode 2: torch's nn.RMSNorm(64, eps) (HunYuanDiTPlain's q/k norms,
+ *         hunyuandit.py:153,256,491): fp16(x * rrms * w) with x * rrms * w in fp32, one rounding, where mode 0 rounds
+ *         x * rrms before the scale.  Other modes are R3G_E_INVALID.  k_w == NULL skips k (geo-decoder query side). */
 int r3g_qk_norm(r3g_ctx* ctx, void* buf, int64_t ld, int rows, int heads, int64_t q_off, int64_t k_off,
                 int64_t head_stride, int mode, float eps, const void* q_w, const void* q_b, const void* k_w,
                 const void* k_b, int seg_len, int64_t seg_stride, void* stream);

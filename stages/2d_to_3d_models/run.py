@@ -39,7 +39,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, os.path.join(ROOT, "3d-re-gen_b200"))
 
 from r3g.dist import MeshBatchGatherer, create_object_groups, plan_object_groups  # noqa: E402
-from r3g.pipelines import Hunyuan3DDiTFlowMatchingPipeline, SimpleMesh  # noqa: E402
+from r3g.pipelines import HUNYUAN3D_2MINI_CONFIG, Hunyuan3DDiTFlowMatchingPipeline, SimpleMesh  # noqa: E402
 from r3g.postprocessors import DegenerateFaceRemover, FaceReducerR3G, FloaterRemover  # noqa: E402
 
 
@@ -81,10 +81,11 @@ def main():
     if not names:
         raise FileNotFoundError(f"No images found in the input folder '{input_folder}'.")
 
-    if args.random_weights:
-        pipe = Hunyuan3DDiTFlowMatchingPipeline.from_random(seed=0, device=f"cuda:{local}")
+    mini = config.get("mini", True)
+    if args.random_weights:     # the architecture `mini` names, with seeded weights
+        pipe = Hunyuan3DDiTFlowMatchingPipeline.from_random(seed=0, device=f"cuda:{local}",
+                                                            config=HUNYUAN3D_2MINI_CONFIG if mini else None)
     else:
-        mini = config.get("mini", True)
         repo = "tencent/Hunyuan3D-2mini" if mini else "tencent/Hunyuan3D-2"
         kw = dict(subfolder="hunyuan3d-dit-v2-mini", variant="fp16") if mini else {}
         pipe = Hunyuan3DDiTFlowMatchingPipeline.from_pretrained(repo, device=f"cuda:{local}", **kw)
