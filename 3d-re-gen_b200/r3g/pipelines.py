@@ -91,6 +91,13 @@ HUNYUAN3D_2MINI_CONFIG = dict(
 # architecture run with CFG and the consistency scheduler (pcm_timesteps = 100 UNVERIFIED, as for 2.0-turbo)
 HUNYUAN3D_2MINI_TURBO_CONFIG = dict(HUNYUAN3D_2MINI_CONFIG, scheduler=HUNYUAN3D_2_TURBO_CONFIG["scheduler"])
 
+# `hunyuan3d-vae-v2-mini-withencoder` (minimal_vae_demo.py): ShapeVAE's constructor arguments, the 2mini VAE above plus
+# the encoder's.  UNVERIFIED: the checkpoint's config.yaml is not in the reference tree; the encoder values are the
+# constructor defaults of model.py:199-223 (5120 + 5120 surface points, as the demo's SharpEdgeSurfaceLoader samples).
+HUNYUAN3D_2MINI_VAE_WITHENCODER_CONFIG = dict(
+    HUNYUAN3D_2MINI_CONFIG["vae"], num_encoder_layers=8, pc_size=5120, pc_sharpedge_size=5120, point_feats=3,
+    downsample_ratio=20, use_ln_post=True)
+
 
 def denoiser_class(target):
     """The denoiser a config's `model.target` names (pipelines.py:121-128 instantiates it).  None: Hunyuan3DDiT, the

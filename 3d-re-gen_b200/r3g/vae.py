@@ -13,8 +13,18 @@ Both extractors run on the GPU.  'mc' is Lewiner marching cubes in scikit-image'
 dual marching cubes (one vertex per connected patch of a cell's Lewiner tiling, one quad per interior sign-changing grid
 edge; include/r3g.h), not diso's DiffDMC, whose vertex rule and output order are not reproduced.
 
-The encoder side (PointCrossAttentionEncoder, pre_kl) is not on the inference path (SURVEY.md section 2, row 12).
+The encoder side, for the `-withencoder` checkpoints (minimal_vae_demo.py):
+
+  ShapeVAE.from_pretrained / from_single_file    VectsetVAE                  model.py:82-141
+  vae.encode(surface, sample_posterior)          ShapeVAE.encode             model.py:284-293
+  vae.encoder                                    PointCrossAttentionEncoder  attention_blocks.py:497-699
+
+Its cross-attention block is the geo decoder's sequence (_cross_kv, _cross_block) and its self-attention blocks the
+decoder transformer's (_attention_blocks) under other key prefixes.  Farthest point sampling is device-side torch.
 """
+import math
+import os
+
 import numpy as np
 import torch
 
@@ -35,6 +45,100 @@ def _h(sd, name, dev, required=True):
             raise KeyError(name)
         return None
     return t.detach().to(device=dev, dtype=torch.float16).contiguous()
+
+
+def _cross_block_weights(g, prefix, qk_norm):
+    """The weights of one ResidualCrossAttentionBlock (attention_blocks.py:264-299) under `prefix`, by the short names
+    _cross_kv and _cross_block read.  g(name, required=True): the fp16 device tensor of a state-dict key."""
+    w = {}
+    for n in ("ln_1", "ln_2", "ln_3"):
+        w[n + ".weight"], w[n + ".bias"] = g(prefix + n + ".weight"), g(prefix + n + ".bias")
+    w["c_q.weight"], w["c_q.bias"] = g(prefix + "attn.c_q.weight"), g(prefix + "attn.c_q.bias", False)
+    w["c_kv.weight"], w["c_kv.bias"] = g(prefix + "attn.c_kv.weight"), g(prefix + "attn.c_kv.bias", False)
+    if qk_norm:
+        for n in ("q_norm", "k_norm"):
+            w[n + ".weight"] = g(prefix + f"attn.attention.{n}.weight")
+            w[n + ".bias"] = g(prefix + f"attn.attention.{n}.bias")
+    for n, r in (("c_proj", "attn.c_proj"), ("c_fc", "mlp.c_fc"), ("mlp_proj", "mlp.c_proj")):
+        w[n + ".weight"], w[n + ".bias"] = g(prefix + r + ".weight"), g(prefix + r + ".bias")
+    return w
+
+
+def _cross_kv(w, data, heads, qk_norm):
+    """ln_2, c_kv and k_norm of a cross-attention block's data rows [n, W]: (kv [n, 2W] laid out (H, (k,v), D), and
+    the k and v views [1, n, H, 64] of it)."""
+    n = data.shape[0]
+    dn = ops.layernorm(data, w["ln_2.weight"], w["ln_2.bias"], eps=1e-6)
+    kv = ops.linear(dn, w["c_kv.weight"], w["c_kv.bias"])
+    if qk_norm:
+        ops.qk_norm_(kv, heads, 0, 0, 128, 1, 1e-6, w["k_norm.weight"], w["k_norm.bias"])
+    kv5 = kv.view(1, n, heads, 2, 64)
+    return kv, kv5[:, :, :, 0], kv5[:, :, :, 1]
+
+
+def _cross_block(w, heads, qk_norm, x, xn, q, h, k, v, attention=None):
+    """x <- x + attn(ln_1(x), data); x <- x + mlp(ln_3(x)), in place on the query rows x [n, W], with k / v the data's
+    projections (_cross_kv).  xn, q [n, W] and h [n, mlp width] are scratch.  attention: optional callable(q4) that
+    replaces the cross attention over all of k / v and leaves its result in q4."""
+    n, W = x.shape
+    ops.layernorm(x, w["ln_1.weight"], w["ln_1.bias"], eps=1e-6, out=xn)
+    if qk_norm:   # per-head LayerNorm of q inside the projection's epilogue
+        ops.linear(xn, w["c_q.weight"], w["c_q.bias"], out=q,
+                   qk_norm=dict(mode=ops.QKN_LAYERNORM, q_col0=0, k_col0=None, cols=W, eps=1e-6,
+                                q_w=w["q_norm.weight"], q_b=w["q_norm.bias"]))
+    else:
+        ops.linear(xn, w["c_q.weight"], w["c_q.bias"], out=q)
+    q4 = q.view(1, n, heads, 64)
+    if attention is None:
+        ops.attention(q4, k, v, out=q4)
+    else:
+        attention(q4)
+    ops.linear(q, w["c_proj.weight"], w["c_proj.bias"], out=x, residual=x)
+    ops.layernorm(x, w["ln_3.weight"], w["ln_3.bias"], eps=1e-6, out=xn)
+    ops.linear(xn, w["c_fc.weight"], w["c_fc.bias"], out=h, act=ops.ACT_GELU_ERF)
+    ops.linear(h, w["mlp_proj.weight"], w["mlp_proj.bias"], out=x, residual=x)
+
+
+def _attention_block_weights(g, prefix, layers, qk_norm):
+    """The weights of the Transformer (attention_blocks.py:398-433) under `prefix`, keyed by their state-dict names
+    (q_norm / k_norm without the `attn.attention.` part)."""
+    w = {}
+    for i in range(layers):
+        p = f"{prefix}resblocks.{i}."
+        for n in ("ln_1", "ln_2", "attn.c_proj", "mlp.c_fc", "mlp.c_proj"):
+            w[p + n + ".weight"], w[p + n + ".bias"] = g(p + n + ".weight"), g(p + n + ".bias")
+        w[p + "attn.c_qkv.weight"] = g(p + "attn.c_qkv.weight")
+        w[p + "attn.c_qkv.bias"] = g(p + "attn.c_qkv.bias", False)
+        if qk_norm:
+            for n in ("q_norm", "k_norm"):
+                w[p + f"{n}.weight"] = g(p + f"attn.attention.{n}.weight")
+                w[p + f"{n}.bias"] = g(p + f"attn.attention.{n}.bias")
+    return w
+
+
+def _attention_blocks(w, prefix, layers, heads, qk_norm, x, taps=None):
+    """The Transformer's `layers` ResidualAttentionBlocks under `prefix`, in place on x [L, W] fp16."""
+    L, W = x.shape
+    xn = torch.empty_like(x)
+    qkv = torch.empty(L, 3 * W, device=x.device, dtype=torch.float16)
+    o = torch.empty(L, W, device=x.device, dtype=torch.float16)
+    h = torch.empty(L, 4 * W, device=x.device, dtype=torch.float16)
+    q5 = qkv.view(1, L, heads, 3, 64)
+    for i in range(layers):
+        p = f"{prefix}resblocks.{i}."
+        ops.layernorm(x, w[p + "ln_1.weight"], w[p + "ln_1.bias"], eps=1e-6, out=xn)
+        ops.linear(xn, w[p + "attn.c_qkv.weight"], w[p + "attn.c_qkv.bias"], out=qkv)
+        if qk_norm:
+            ops.qk_norm_(qkv, heads, 0, 64, 192, 1, 1e-6, w[p + "q_norm.weight"], w[p + "q_norm.bias"],
+                         w[p + "k_norm.weight"], w[p + "k_norm.bias"])
+        ops.attention(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], out=o.view(1, L, heads, 64))
+        ops.linear(o, w[p + "attn.c_proj.weight"], w[p + "attn.c_proj.bias"], out=x, residual=x)
+        ops.layernorm(x, w[p + "ln_2.weight"], w[p + "ln_2.bias"], eps=1e-6, out=xn)
+        ops.linear(xn, w[p + "mlp.c_fc.weight"], w[p + "mlp.c_fc.bias"], out=h, act=ops.ACT_GELU_ERF)
+        ops.linear(h, w[p + "mlp.c_proj.weight"], w[p + "mlp.c_proj.bias"], out=x, residual=x)
+        if taps is not None:
+            taps.append(x.clone())
+    return x
 
 
 class CrossAttentionDecoder:
@@ -66,17 +170,7 @@ class CrossAttentionDecoder:
         pad = torch.zeros(W, 64, device=dev, dtype=torch.float16)  # K = 3+6F = 51 -> 64 (TMA rows of 128 B)
         pad[:, :qp.shape[1]] = qp
         w["query_proj.weight"], w["query_proj.bias"] = pad, g("query_proj.bias")
-        ca = "cross_attn_decoder."
-        for n in ("ln_1", "ln_2", "ln_3"):
-            w[n + ".weight"], w[n + ".bias"] = g(ca + n + ".weight"), g(ca + n + ".bias")
-        w["c_q.weight"], w["c_q.bias"] = g(ca + "attn.c_q.weight"), g(ca + "attn.c_q.bias", False)
-        w["c_kv.weight"], w["c_kv.bias"] = g(ca + "attn.c_kv.weight"), g(ca + "attn.c_kv.bias", False)
-        if self.qk_norm:
-            for n in ("q_norm", "k_norm"):
-                w[n + ".weight"] = g(ca + f"attn.attention.{n}.weight")
-                w[n + ".bias"] = g(ca + f"attn.attention.{n}.bias")
-        for n, r in (("c_proj", ca + "attn.c_proj"), ("c_fc", ca + "mlp.c_fc"), ("mlp_proj", ca + "mlp.c_proj")):
-            w[n + ".weight"], w[n + ".bias"] = g(r + ".weight"), g(r + ".bias")
+        w.update(_cross_block_weights(g, "cross_attn_decoder.", self.qk_norm))
         w["ln_post.weight"], w["ln_post.bias"] = g("ln_post.weight"), g("ln_post.bias")
         w["output_proj.weight"], w["output_proj.bias"] = g("output_proj.weight").view(-1), g("output_proj.bias")
         self.w = w
@@ -85,14 +179,7 @@ class CrossAttentionDecoder:
     # K/V of the latents: projected ONCE per object (the reference re-projects them for every chunk,
     # attention_blocks.py:250-258 with kv_cache=False)
     def _project_kv(self, latents):
-        w, W, nh = self.w, self.width, self.heads
-        n_lat = latents.shape[1]
-        lat_n = ops.layernorm(latents[0], w["ln_2.weight"], w["ln_2.bias"], eps=1e-6)
-        kv = ops.linear(lat_n, w["c_kv.weight"], w["c_kv.bias"])            # [n_lat, 2W] laid out (H, (k,v), D)
-        if self.qk_norm:
-            ops.qk_norm_(kv, nh, 0, 0, 128, 1, 1e-6, w["k_norm.weight"], w["k_norm.bias"])
-        kv5 = kv.view(1, n_lat, nh, 2, 64)
-        return kv, kv5[:, :, :, 0], kv5[:, :, :, 1]
+        return _cross_kv(self.w, latents[0], self.heads, self.qk_norm)
 
     def _workspace(self, n):
         ws = self._ws.get(n)
@@ -107,26 +194,11 @@ class CrossAttentionDecoder:
         """ws['emb'][:n] holds the embedded queries; writes n fp16-rounded logits (as float32) to out_f32[:n].
         attention: optional callable(q4) that replaces the plain cross attention over all latents (FlashVDM's
         top-k key/value selection, attention_processors.py:35-79); it must leave its result in q4."""
-        w, W, nh = self.w, self.width, self.heads
+        w = self.w
         k, v = (kv[1], kv[2]) if kv is not None else (None, None)
         emb, x, xn, q, h = (ws[k_][:n] for k_ in ("emb", "x", "xn", "q", "h"))
         ops.linear(emb, w["query_proj.weight"], w["query_proj.bias"], out=x)
-        ops.layernorm(x, w["ln_1.weight"], w["ln_1.bias"], eps=1e-6, out=xn)
-        if self.qk_norm:   # per-head LayerNorm of q inside the projection's epilogue
-            ops.linear(xn, w["c_q.weight"], w["c_q.bias"], out=q,
-                       qk_norm=dict(mode=ops.QKN_LAYERNORM, q_col0=0, k_col0=None, cols=W, eps=1e-6,
-                                    q_w=w["q_norm.weight"], q_b=w["q_norm.bias"]))
-        else:
-            ops.linear(xn, w["c_q.weight"], w["c_q.bias"], out=q)
-        q4 = q.view(1, n, nh, 64)
-        if attention is None:
-            ops.attention(q4, k, v, out=q4)
-        else:
-            attention(q4)
-        ops.linear(q, w["c_proj.weight"], w["c_proj.bias"], out=x, residual=x)
-        ops.layernorm(x, w["ln_3.weight"], w["ln_3.bias"], eps=1e-6, out=xn)
-        ops.linear(xn, w["c_fc.weight"], w["c_fc.bias"], out=h, act=ops.ACT_GELU_ERF)
-        ops.linear(h, w["mlp_proj.weight"], w["mlp_proj.bias"], out=x, residual=x)
+        _cross_block(w, self.heads, self.qk_norm, x, xn, q, h, k, v, attention)
         ops.lnpost_dot(x, w["ln_post.weight"], w["ln_post.bias"], w["output_proj.weight"], w["output_proj.bias"],
                        out_f32, eps=1e-5)
 
@@ -473,6 +545,187 @@ class DMCSurfaceExtractor(SurfaceExtractor):
 SurfaceExtractors = {"mc": MCSurfaceExtractor, "dmc": DMCSurfaceExtractor}
 
 
+def fps_count(n, ratio):
+    """Points torch_cluster.fps keeps of an n-point batch segment at `ratio`: ceil(n * ratio), the product taken in
+    float32 (the ratio is a float32 tensor there).  UNVERIFIED against torch_cluster, which is not installed here."""
+    return int(math.ceil(float(np.float32(n) * np.float32(ratio))))
+
+
+def farthest_point_sample(points, start, count):
+    """Farthest point sampling of every batch segment: points float32 [B, n, 3], start int64 [B] (the first pick of
+    each segment) -> int64 [B, count] indices within the segments.  Pick i + 1 is the point whose float32 squared
+    distance to the picks so far is largest (dx*dx + dy*dy, then + dz*dz, each operation rounded), the lowest index
+    among equal distances.  Device-side torch operations with no host synchronisation, so a CUDA graph captures the
+    loop; each pick costs seven small kernels."""
+    B, n, _ = points.shape
+    idx = torch.empty(count, B, device=points.device, dtype=torch.long)
+    idx[0] = start
+    dist = torch.full((B, n), float("inf"), device=points.device, dtype=torch.float32)
+    diff = torch.empty_like(points)
+    d = torch.empty(B, n, device=points.device, dtype=torch.float32)
+    for i in range(1, count):
+        last = points.gather(1, idx[i - 1].view(B, 1, 1).expand(B, 1, 3))
+        torch.sub(points, last, out=diff)
+        diff.mul_(diff)
+        torch.add(diff[..., 0], diff[..., 1], out=d)
+        d.add_(diff[..., 2])
+        torch.minimum(dist, d, out=dist)
+        torch.argmax(dist, dim=1, out=idx[i])
+    return idx.t().contiguous()
+
+
+class PointCrossAttentionEncoder:
+    """The ShapeVAE encoder (attention_blocks.py:511-699) on the r3g kernels: the reference's random / sharp-edge
+    split of the surface points, a randperm subset of each part and its farthest-point-sampled queries
+    (sample_points_and_latents), the Fourier embedding with the point features appended, input_proj, one
+    ResidualCrossAttentionBlock of the queries over all subset points, `layers` self-attention blocks and ln_post.
+
+    The random draws (two permutations, the FPS start points) are arguments of `sample` and `forward`, so that a
+    caller can pin them; `draw` makes them the way the reference does."""
+
+    def __init__(self, *, num_latents, downsample_ratio, pc_size, pc_sharpedge_size, point_feats, width, heads, layers,
+                 num_freqs=8, include_pi=True, normal_pe=False, qkv_bias=True, use_ln_post=False, qk_norm=False,
+                 device="cuda"):
+        if normal_pe:
+            raise NotImplementedError("normal_pe=True (Fourier features of the normals) is not mirrored: the "
+                                      "Hunyuan3D-2 ShapeVAE never sets it")
+        if width // heads != 64:
+            raise ValueError("r3g attention kernels are built for head_dim 64")
+        self.num_latents, self.downsample_ratio = num_latents, downsample_ratio
+        self.pc_size, self.pc_sharpedge_size, self.point_feats = pc_size, pc_sharpedge_size, point_feats
+        self.width, self.heads, self.layers = width, heads, layers
+        self.num_freqs, self.include_pi = num_freqs, include_pi
+        self.qkv_bias, self.use_ln_post, self.qk_norm = qkv_bias, use_ln_post, qk_norm
+        self.device = torch.device(device)
+        self.in_dim = 3 + 6 * num_freqs + point_feats       # FourierEmbedder.out_dim + point_feats
+        self.k_pad = -(-self.in_dim // 64) * 64               # input_proj's K, zero padded (TMA rows of 128 B)
+        self.w = None
+
+    def load(self, sd, prefix="encoder."):
+        dev, W = self.device, self.width
+        g = lambda n, req=True: _h(sd, prefix + n, dev, req)  # noqa: E731
+        ip = g("input_proj.weight")
+        if ip.shape != (W, self.in_dim):
+            raise ValueError(f"{prefix}input_proj.weight is {tuple(ip.shape)}, the config gives {(W, self.in_dim)}")
+        pad = torch.zeros(W, self.k_pad, device=dev, dtype=torch.float16)
+        pad[:, :self.in_dim] = ip
+        w = {"input_proj.weight": pad, "input_proj.bias": g("input_proj.bias")}
+        w.update(_cross_block_weights(g, "cross_attn.", self.qk_norm))
+        w.update(_attention_block_weights(g, "self_attn.", self.layers, self.qk_norm))
+        if self.use_ln_post:
+            w["ln_post.weight"], w["ln_post.bias"] = g("ln_post.weight"), g("ln_post.bias")
+        self.w = w
+        return self
+
+    def plan(self):
+        """(subset size, FPS ratio, queries) of the random part, then of the sharp-edge part: the arithmetic of
+        attention_blocks.py:576-610 (a part whose subset size is 0 has ratio None and no queries).  The query counts
+        come from the nominal subset sizes and need not add up to num_latents (ceil: 17 for 16 latents over a
+        300 / 200 split).  A subset larger than its part raises, as the reference's view of the subset does."""
+        num_latents = int(self.num_latents * self.downsample_ratio / self.downsample_ratio)
+        n_rand_q = self.pc_size / (self.pc_size + self.pc_sharpedge_size) * num_latents
+        n_sharp_q = num_latents - n_rand_q
+        parts = []
+        for nq, size, name in ((n_rand_q, self.pc_size, "pc_size"), (n_sharp_q, self.pc_sharpedge_size,
+                                                                    "pc_sharpedge_size")):
+            n = int(nq * self.downsample_ratio)
+            if n > size:
+                raise ValueError(f"the encoder draws {n} points from the {size} of {name}: {name} must be at least "
+                                 "num_latents * downsample_ratio times its share of the surface")
+            ratio = nq / n if n else None
+            parts.append((n, ratio, fps_count(n, ratio) if n else 0))
+        return tuple(parts)
+
+    def queries(self):
+        (_, _, m_r), (_, _, m_s) = self.plan()
+        return m_r + m_s
+
+    def draw(self, surface):
+        """The reference's random draws, in its order, on the surface's device: randperm of the random part, the FPS
+        start of each batch segment (torch_cluster: int64(rand() * n), UNVERIFIED), then the same for the sharp-edge
+        part when it has a subset.  Returns (perm_r, start_r, perm_s, start_s); an empty part gets an empty
+        permutation and zero starts, drawing nothing."""
+        B, dev = surface.shape[0], surface.device
+        (n_r, _, _), (n_s, _, _) = self.plan()
+        perm_r = torch.randperm(self.pc_size, device=dev)
+        start_r = (torch.rand(B, device=dev) * n_r).long()
+        if n_s == 0:
+            return perm_r, start_r, torch.empty(0, device=dev, dtype=torch.long), torch.zeros_like(start_r)
+        perm_s = torch.randperm(self.pc_sharpedge_size, device=dev)
+        start_s = (torch.rand(B, device=dev) * n_s).long()
+        return perm_r, start_r, perm_s, start_s
+
+    def sample(self, surface, perm_r, start_r, perm_s, start_s):
+        """sample_points_and_latents on given draws.  surface fp16 [B, pc_size + pc_sharpedge_size, 3 + point_feats];
+        perm_*: a permutation of the part's points (its first subset-size entries are used), start_*: int64 [B].
+        Returns (query rows [B, Lq, 3 + point_feats], data rows [B, Nd, 3 + point_feats], FPS picks of each part as
+        indices into its flattened [B * subset, ...] rows, torch_cluster.fps's output)."""
+        B, N, D = surface.shape
+        if N != self.pc_size + self.pc_sharpedge_size or D != 3 + self.point_feats:
+            raise ValueError(f"surface must be [B, {self.pc_size + self.pc_sharpedge_size}, {3 + self.point_feats}], "
+                             f"got {tuple(surface.shape)}")
+        queries, data, picks = [], [], []
+        for (n, _, m), part, perm, start in zip(self.plan(), (surface[:, :self.pc_size], surface[:, self.pc_size:]),
+                                                (perm_r, perm_s), (start_r, start_s)):
+            if n == 0:
+                picks.append(torch.empty(0, device=surface.device, dtype=torch.long))
+                continue
+            sub = part.index_select(1, perm[:n])                                   # [B, n, D]
+            local = farthest_point_sample(sub[..., :3].float(), start, m)           # [B, m]
+            flat = (local + torch.arange(B, device=surface.device)[:, None] * n).view(-1)
+            queries.append(sub.reshape(B * n, D).index_select(0, flat).view(B, m, D))
+            data.append(sub)
+            picks.append(flat)
+        return torch.cat(queries, 1), torch.cat(data, 1), picks
+
+    def _embed(self, rows):
+        """Fourier features of the points with the point features appended, zero padded: [n, k_pad] fp16."""
+        emb = torch.empty(rows.shape[0], self.k_pad, device=rows.device, dtype=torch.float16)
+        ops.points_fourier(rows[:, :3], emb, self.num_freqs, self.include_pi)
+        if self.point_feats:
+            emb[:, 3 + 6 * self.num_freqs:self.in_dim].copy_(rows[:, 3:])
+        return emb
+
+    def forward(self, query_rows, data_rows):
+        """The network on one object's sampled rows (sample): [Lq, 3 + point_feats], [Nd, ...] fp16 -> latents
+        [Lq, width] fp16."""
+        w, nh, W = self.w, self.heads, self.width
+        x = ops.linear(self._embed(query_rows), w["input_proj.weight"], w["input_proj.bias"])
+        data = ops.linear(self._embed(data_rows), w["input_proj.weight"], w["input_proj.bias"])
+        _, k, v = _cross_kv(w, data, nh, self.qk_norm)
+        L = x.shape[0]
+        xn, q = torch.empty_like(x), torch.empty_like(x)
+        h = torch.empty(L, 4 * W, device=x.device, dtype=torch.float16)
+        _cross_block(w, nh, self.qk_norm, x, xn, q, h, k, v)
+        _attention_blocks(w, "self_attn.", self.layers, nh, self.qk_norm, x)
+        if self.use_ln_post:
+            ops.layernorm(x, w["ln_post.weight"], w["ln_post.bias"], eps=1e-5, out=xn)
+            return xn
+        return x
+
+
+def diagonal_gaussian(moments, noise=None):
+    """DiagonalGaussianDistribution(moments, feat_dim=-1) (model.py:30-50) in the moments' dtype: (mean, clamped
+    logvar, sample), the sample being mean + exp(0.5 * logvar) * noise, or the mean when noise is None (mode())."""
+    mean, logvar = torch.chunk(moments, 2, dim=-1)
+    logvar = torch.clamp(logvar, -30.0, 20.0)
+    if noise is None:
+        return mean, logvar, mean
+    return mean, logvar, mean + torch.exp(0.5 * logvar) * noise
+
+
+class _SeenKeys(dict):
+    """A state dict that records the keys read through get() into `seen` (ShapeVAE.load_state_dict's strict check)."""
+
+    def __init__(self, sd, seen):
+        super().__init__(sd)
+        self.seen = seen
+
+    def get(self, key, default=None):
+        self.seen.add(key)
+        return super().get(key, default)
+
+
 class ShapeVAE:
     def __init__(self, *, num_latents, embed_dim, width, heads, num_decoder_layers, num_encoder_layers=8,
                  pc_size=5120, pc_sharpedge_size=5120, point_feats=3, downsample_ratio=20,
@@ -492,10 +745,56 @@ class ShapeVAE:
         self.device = torch.device(device)
         self.geo_decoder = CrossAttentionDecoder(width, heads, num_freqs, include_pi, geo_decoder_mlp_expand_ratio,
                                                  qk_norm, geo_decoder_ln_post, device)
+        self.encoder = PointCrossAttentionEncoder(
+            num_latents=num_latents, downsample_ratio=downsample_ratio, pc_size=pc_size,
+            pc_sharpedge_size=pc_sharpedge_size, point_feats=point_feats, width=width, heads=heads,
+            layers=num_encoder_layers, num_freqs=num_freqs, include_pi=include_pi, qkv_bias=qkv_bias,
+            use_ln_post=use_ln_post, qk_norm=qk_norm, device=device)
         self.volume_decoder = volume_decoder if volume_decoder is not None else VanillaVolumeDecoder()
         self.surface_extractor = surface_extractor if surface_extractor is not None else MCSurfaceExtractor()
         self.w = None
         self.taps = None
+        self.has_encoder = False
+        self.use_cuda_graph = True
+        self._enc_graphs = GraphCache(keep_all=True)    # one encode graph per (surface shape, sampled or not)
+
+    @classmethod
+    def from_single_file(cls, ckpt_path, config_path, device="cuda", dtype=torch.float16, use_safetensors=None,
+                         **kwargs):
+        """model.py:82-114: a config.yaml whose `params` are the constructor's arguments (kwargs override them) and a
+        checkpoint holding the flat state dict, loaded with strict=False as there."""
+        import yaml
+        if dtype != torch.float16:
+            raise NotImplementedError(f"dtype {dtype}: the r3g kernels run the ShapeVAE in float16")
+        with open(config_path) as fh:
+            config = yaml.safe_load(fh)
+        if use_safetensors:
+            ckpt_path = ckpt_path.replace(".ckpt", ".safetensors")
+        if not os.path.exists(ckpt_path):
+            raise FileNotFoundError(f"Model file {ckpt_path} not found")
+        if use_safetensors:
+            import safetensors.torch
+            ckpt = safetensors.torch.load_file(ckpt_path, device="cpu")
+        else:
+            ckpt = torch.load(ckpt_path, map_location="cpu", weights_only=True)
+        model_kwargs = dict(config["params"])
+        model_kwargs.update(kwargs)
+        return cls(device=device, **model_kwargs).load_state_dict(ckpt, strict=False)
+
+    @classmethod
+    def from_pretrained(cls, model_path, device="cuda", dtype=torch.float16, use_safetensors=True, variant="fp16",
+                        subfolder="hunyuan3d-vae-v2-0", **kwargs):
+        """model.py:116-141 + utils.py:89-126: `model{.variant}.{safetensors|ckpt}` and `config.yaml` under
+        $HY3DGEN_MODELS (default ~/.cache/hy3dgen)/model_path/subfolder.  The reference would fall back to a
+        HuggingFace download, which needs a network this build does not have."""
+        base = os.path.expanduser(os.path.join(os.environ.get("HY3DGEN_MODELS", "~/.cache/hy3dgen"), model_path,
+                                               subfolder))
+        if not os.path.isdir(base):
+            raise FileNotFoundError(f"{base} not found and no network for snapshot_download")
+        ext = "safetensors" if use_safetensors else "ckpt"
+        vs = "" if variant is None else f".{variant}"
+        return cls.from_single_file(os.path.join(base, f"model{vs}.{ext}"), os.path.join(base, "config.yaml"),
+                                    device=device, dtype=dtype, use_safetensors=use_safetensors, **kwargs)
 
     def to(self, *a, **k):
         return self
@@ -504,24 +803,35 @@ class ShapeVAE:
         return self
 
     def load_state_dict(self, sd, strict=False):
+        """The decoder side always; `encoder.*` and `pre_kl.*` when the checkpoint has encoder keys (the
+        `-withencoder` checkpoints), else encode() is refused.  strict=True also refuses a checkpoint without the
+        encoder and any key the reference ShapeVAE does not have."""
         dev = self.device
-        w = {"post_kl.weight": _h(sd, "post_kl.weight", dev), "post_kl.bias": _h(sd, "post_kl.bias", dev)}
-        for i in range(self.layers):
-            p = f"transformer.resblocks.{i}."
-            for n in ("ln_1", "ln_2", "attn.c_proj", "mlp.c_fc", "mlp.c_proj"):
-                w[p + n + ".weight"], w[p + n + ".bias"] = _h(sd, p + n + ".weight", dev), _h(sd, p + n + ".bias", dev)
-            w[p + "attn.c_qkv.weight"] = _h(sd, p + "attn.c_qkv.weight", dev)
-            w[p + "attn.c_qkv.bias"] = _h(sd, p + "attn.c_qkv.bias", dev, False)
-            if self.qk_norm:
-                for n in ("q_norm", "k_norm"):
-                    w[p + f"{n}.weight"] = _h(sd, p + f"attn.attention.{n}.weight", dev)
-                    w[p + f"{n}.bias"] = _h(sd, p + f"attn.attention.{n}.bias", dev)
+        seen = set()
+
+        def g(name, required=True):
+            seen.add(name)
+            return _h(sd, name, dev, required)
+        w = {"post_kl.weight": g("post_kl.weight"), "post_kl.bias": g("post_kl.bias")}
+        w.update(_attention_block_weights(g, "transformer.", self.layers, self.qk_norm))
+        self.geo_decoder.load(_SeenKeys(sd, seen))
+        self.has_encoder = any(k.startswith("encoder.") for k in sd)
+        if self.has_encoder:
+            w["pre_kl.weight"], w["pre_kl.bias"] = g("pre_kl.weight"), g("pre_kl.bias")
+            self.encoder.load(_SeenKeys(sd, seen))
+        if strict:
+            if not self.has_encoder:
+                raise RuntimeError("strict load: the checkpoint has no encoder.* keys")
+            unexpected = sorted(k for k in sd if k not in seen)
+            if unexpected:
+                raise RuntimeError(f"strict load: unexpected keys {unexpected[:5]}")
         self.w = w
-        self.geo_decoder.load(sd)
         self._ref_sd = sd
         return self
 
-    def init_random(self, seed=0, std=0.02):
+    def init_random(self, seed=0, std=0.02, encoder=False):
+        """Seeded random weights in the reference's key layout; encoder=True adds the encoder and pre_kl (drawn after
+        the decoder's weights, which are the same either way)."""
         gen = torch.Generator(device="cpu").manual_seed(seed)
         W, Mw = self.width, self.width * 4
         sd = {}
@@ -558,6 +868,30 @@ class ShapeVAE:
         lin(ca + "mlp.c_proj", W, self.geo_decoder.mlp_width)
         ln(g + "ln_post", W)
         lin(g + "output_proj", 1, W, s=0.3)
+        if encoder:
+            e = "encoder."
+            lin(e + "input_proj", W, self.encoder.in_dim, s=0.3)
+            c = e + "cross_attn."
+            ln(c + "ln_1", W); ln(c + "ln_2", W); ln(c + "ln_3", W)
+            lin(c + "attn.c_q", W, W, self.qkv_bias)
+            lin(c + "attn.c_kv", 2 * W, W, self.qkv_bias)
+            if self.qk_norm:
+                ln(c + "attn.attention.q_norm", 64); ln(c + "attn.attention.k_norm", 64)
+            lin(c + "attn.c_proj", W, W)
+            lin(c + "mlp.c_fc", Mw, W)
+            lin(c + "mlp.c_proj", W, Mw)
+            for i in range(self.encoder.layers):
+                p = f"{e}self_attn.resblocks.{i}."
+                ln(p + "ln_1", W); ln(p + "ln_2", W)
+                lin(p + "attn.c_qkv", 3 * W, W, self.qkv_bias)
+                lin(p + "attn.c_proj", W, W)
+                lin(p + "mlp.c_fc", Mw, W)
+                lin(p + "mlp.c_proj", W, Mw)
+                if self.qk_norm:
+                    ln(p + "attn.attention.q_norm", 64); ln(p + "attn.attention.k_norm", 64)
+            if self.encoder.use_ln_post:
+                ln(e + "ln_post", W)
+            lin("pre_kl", 2 * self.embed_dim, W)
         return self.load_state_dict(sd)
 
     def reference_state_dict(self):
@@ -566,35 +900,60 @@ class ShapeVAE:
     @torch.no_grad()
     def forward(self, latents):
         """post_kl + transformer; latents [B, num_latents, embed_dim] fp16 -> [B, num_latents, width] fp16."""
-        w, W, nh = self.w, self.width, self.heads
-        B, L, _ = latents.shape
+        w = self.w
+        B = latents.shape[0]
         outs = []
         for b in range(B):
             x = ops.linear(latents[b].contiguous(), w["post_kl.weight"], w["post_kl.bias"])
-            xn = torch.empty_like(x)
-            qkv = torch.empty(L, 3 * W, device=x.device, dtype=torch.float16)
-            o = torch.empty(L, W, device=x.device, dtype=torch.float16)
-            h = torch.empty(L, 4 * W, device=x.device, dtype=torch.float16)
-            q5 = qkv.view(1, L, nh, 3, 64)
-            for i in range(self.layers):
-                p = f"transformer.resblocks.{i}."
-                ops.layernorm(x, w[p + "ln_1.weight"], w[p + "ln_1.bias"], eps=1e-6, out=xn)
-                ops.linear(xn, w[p + "attn.c_qkv.weight"], w[p + "attn.c_qkv.bias"], out=qkv)
-                if self.qk_norm:
-                    ops.qk_norm_(qkv, nh, 0, 64, 192, 1, 1e-6, w[p + "q_norm.weight"], w[p + "q_norm.bias"],
-                                 w[p + "k_norm.weight"], w[p + "k_norm.bias"])
-                ops.attention(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], out=o.view(1, L, nh, 64))
-                ops.linear(o, w[p + "attn.c_proj.weight"], w[p + "attn.c_proj.bias"], out=x, residual=x)
-                ops.layernorm(x, w[p + "ln_2.weight"], w[p + "ln_2.bias"], eps=1e-6, out=xn)
-                ops.linear(xn, w[p + "mlp.c_fc.weight"], w[p + "mlp.c_fc.bias"], out=h, act=ops.ACT_GELU_ERF)
-                ops.linear(h, w[p + "mlp.c_proj.weight"], w[p + "mlp.c_proj.bias"], out=x, residual=x)
-                if self.taps is not None:
-                    self.taps.append(x.clone())
-            outs.append(x)
+            outs.append(_attention_blocks(w, "transformer.", self.layers, self.heads, self.qk_norm, x, self.taps))
         return torch.stack(outs, 0)
 
     __call__ = forward
     decode = forward
+
+    @torch.no_grad()
+    def encode(self, surface, sample_posterior=True):
+        """model.py:284-293: surface fp16 [B, pc_size + pc_sharpedge_size, 3 + point_feats] (xyz | point features,
+        the random part first) -> latents [B, Lq, embed_dim] fp16, a sample of the posterior or its mean.  Draws
+        the reference's random choices on the surface's device (PointCrossAttentionEncoder.draw, then the posterior
+        noise) and runs encode_core on them."""
+        self._check_encoder(surface)
+        draws = self.encoder.draw(surface)
+        noise = None
+        if sample_posterior:
+            noise = torch.randn(surface.shape[0], self.encoder.queries(), self.embed_dim, device=surface.device,
+                                dtype=torch.float16)
+        return self.encode_core(surface, *draws, noise=noise)[0]
+
+    def _check_encoder(self, surface):
+        if not self.has_encoder:
+            raise RuntimeError("encode() needs a checkpoint with the encoder (a `-withencoder` ShapeVAE): the loaded "
+                               "state dict has no encoder.* keys")
+        if surface.dtype != torch.float16:
+            raise TypeError(f"surface must be float16, as the reference's fp16 ShapeVAE takes it; got {surface.dtype}")
+
+    @torch.no_grad()
+    def encode_core(self, surface, perm_r, start_r, perm_s, start_s, noise=None):
+        """encode on given draws (PointCrossAttentionEncoder.draw): returns (latents, mean, logvar, FPS picks of the
+        random part, of the sharp-edge part) -- latents = mean + exp(0.5 logvar) * noise, or the mean without noise.
+        On a CUDA device the whole of it, FPS included, is one CUDA graph per surface shape, replayed."""
+        self._check_encoder(surface)
+        surface = surface.contiguous()
+        ins = (surface, perm_r, start_r, perm_s, start_s) + (() if noise is None else (noise,))
+        if not self.use_cuda_graph or surface.device.type != "cuda":
+            return self._encode_eager(*ins)
+        g = self._enc_graphs.get((tuple(surface.shape), noise is not None), ins, self._encode_eager)
+        for dst, src in zip(g.inputs, ins):
+            dst.copy_(src)
+        g.replay()
+        return tuple(t.clone() for t in g.outputs)
+
+    def _encode_eager(self, surface, perm_r, start_r, perm_s, start_s, noise=None):
+        queries, data, (pick_r, pick_s) = self.encoder.sample(surface, perm_r, start_r, perm_s, start_s)
+        moments = torch.stack([ops.linear(self.encoder.forward(queries[b], data[b]), self.w["pre_kl.weight"],
+                                          self.w["pre_kl.bias"]) for b in range(surface.shape[0])])
+        mean, logvar, latents = diagonal_gaussian(moments, noise)
+        return latents.contiguous(), mean.contiguous(), logvar.contiguous(), pick_r, pick_s
 
     def latents2mesh(self, latents, **kwargs):
         grid_logits = self.volume_decoder(latents, self.geo_decoder, **kwargs)
