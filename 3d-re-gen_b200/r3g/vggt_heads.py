@@ -166,13 +166,33 @@ def _uv_embed(x, W, H, ratio=0.1):
     return x + (emb * ratio).permute(2, 0, 1)[None]
 
 
+def _activate(fmap, activation, conf_activation):
+    """activate_head (heads/head_act.py) on a channels-last [..., output_dim] map -> (points [..., output_dim - 1],
+    confidence [...])."""
+    xyz, conf = fmap[..., :-1], fmap[..., -1]
+    if activation == "exp":
+        pts = torch.exp(xyz)
+    elif activation == "inv_log":
+        pts = torch.sign(xyz) * torch.expm1(torch.abs(xyz))
+    else:
+        raise ValueError(f"Unknown activation: {activation}")
+    return pts, (1 + conf.exp() if conf_activation == "expp1" else conf.exp())
+
+
 class DPTHead:
+    """DPTHead (dpt_head.py) as torch operators, in VGGT's three configurations: the depth head (output_dim 2, "exp"),
+    the point head (output_dim 4, "inv_log") and the track head's feature extractor (feature_only=True, down_ratio=2,
+    pos_embed=False), which stops after output_conv1 and the upsample to (H, W) / down_ratio and returns
+    [B, S, features, H / 2, W / 2].  The output width is that of the output_conv2.2 weight."""
+
     def __init__(self, sd, prefix="depth_head.", patch_size=14, activation="exp", conf_activation="expp1",
-                 intermediate_layer_idx=(4, 11, 17, 23), pos_embed=True, device="cuda"):
+                 intermediate_layer_idx=(4, 11, 17, 23), pos_embed=True, feature_only=False, down_ratio=1,
+                 device="cuda"):
         self.sd = {k[len(prefix):]: v.detach().to(device=device, dtype=torch.float32) for k, v in sd.items()
                    if k.startswith(prefix)}
         self.patch_size, self.activation, self.conf_activation = patch_size, activation, conf_activation
         self.layers, self.pos_embed = tuple(intermediate_layer_idx), pos_embed
+        self.feature_only, self.down_ratio = feature_only, down_ratio
 
     def _conv(self, name, x, **kw):
         return F.conv2d(x, self.sd[name + ".weight"], self.sd.get(name + ".bias"), **kw)
@@ -197,12 +217,11 @@ class DPTHead:
         B, S, _, H, W = images.shape
         if frames_chunk_size is None or frames_chunk_size >= S:
             return self._impl(aggregated_tokens_list, H, W, B, S, patch_start_idx, 0, S)
-        preds, confs = [], []
-        for s0 in range(0, S, frames_chunk_size):
-            pr, cf = self._impl(aggregated_tokens_list, H, W, B, S, patch_start_idx, s0, min(s0 + frames_chunk_size, S))
-            preds.append(pr)
-            confs.append(cf)
-        return torch.cat(preds, 1), torch.cat(confs, 1)
+        chunks = [self._impl(aggregated_tokens_list, H, W, B, S, patch_start_idx, s0, min(s0 + frames_chunk_size, S))
+                  for s0 in range(0, S, frames_chunk_size)]
+        if self.feature_only:
+            return torch.cat(chunks, 1)
+        return torch.cat([c[0] for c in chunks], 1), torch.cat([c[1] for c in chunks], 1)
 
     def _impl(self, tokens, H, W, B, S_all, psi, s0, s1):
         sd, S = self.sd, s1 - s0
@@ -227,19 +246,14 @@ class DPTHead:
         out = self._fuse("scratch.refinenet2.", out, l2, size=l1.shape[2:])
         out = self._fuse("scratch.refinenet1.", out, l1)
         out = self._conv("scratch.output_conv1", out, padding=1)
-        out = F.interpolate(out, size=(ph * self.patch_size, pw * self.patch_size), mode="bilinear", align_corners=True)
+        size = (int(ph * self.patch_size / self.down_ratio), int(pw * self.patch_size / self.down_ratio))
+        out = F.interpolate(out, size=size, mode="bilinear", align_corners=True)
         if self.pos_embed:
             out = _uv_embed(out, W, H)
+        if self.feature_only:
+            return out.view(B, S, *out.shape[1:])
         out = self._conv("scratch.output_conv2.2", F.relu(self._conv("scratch.output_conv2.0", out, padding=1)))
-        fmap = out.permute(0, 2, 3, 1)
-        xyz, conf = fmap[..., :-1], fmap[..., -1]
-        if self.activation == "exp":
-            pts = torch.exp(xyz)
-        elif self.activation == "inv_log":
-            pts = torch.sign(xyz) * torch.expm1(torch.abs(xyz))
-        else:
-            raise ValueError(f"Unknown activation: {self.activation}")
-        cf = 1 + conf.exp() if self.conf_activation == "expp1" else conf.exp()
+        pts, cf = _activate(out.permute(0, 2, 3, 1), self.activation, self.conf_activation)
         return pts.view(B, S, *pts.shape[1:]), cf.view(B, S, *cf.shape[1:])
 
 
@@ -250,16 +264,21 @@ class DPTHeadR3G:
     resampling `ops.bilinear_nhwc`; the token LayerNorm is `ops.layernorm_f32in`.  The reference runs this head in float32
     outside autocast on cuDNN; here operands are fp16 with float32 accumulation (parity: rel-L2 <= 1e-2 on depth and
     confidence against the float32 mirror).  Element-wise glue (the in-place ReLU of the residual units, adding two feature
-    maps, the UV position embedding, exp) stays torch.  One CUDA graph per (frames, H, W)."""
+    maps, the UV position embedding, exp) stays torch.  One CUDA graph per (frames, H, W).  The point head's 1x1
+    output_conv2.2 has 4 output rows, zero-padded to 32 like every other convolution's.  With feature_only=True (the
+    track head's feature extractor) the result is the fp16 channels-last map [B, S, H / down_ratio, W / down_ratio,
+    features] that the tracker reads."""
 
     def __init__(self, sd, prefix="depth_head.", patch_size=14, activation="exp", conf_activation="expp1",
-                 intermediate_layer_idx=(4, 11, 17, 23), pos_embed=True, device="cuda"):
+                 intermediate_layer_idx=(4, 11, 17, 23), pos_embed=True, feature_only=False, down_ratio=1,
+                 device="cuda"):
         from . import ops
         self.ops = ops
         dev = self.device = torch.device(device)
         raw = {k[len(prefix):]: v.detach().to(dev) for k, v in sd.items() if k.startswith(prefix)}
         self.patch_size, self.activation, self.conf_activation = patch_size, activation, conf_activation
         self.layers, self.pos_embed = tuple(intermediate_layer_idx), pos_embed
+        self.feature_only, self.down_ratio = feature_only, down_ratio
         h = lambda t: t.to(torch.float16).contiguous()  # noqa: E731
         w = {"norm.weight": h(raw["norm.weight"]), "norm.bias": h(raw["norm.bias"])}
 
@@ -298,8 +317,9 @@ class DPTHeadR3G:
                 conv(f"{p}resConfUnit{u}.conv1")
                 conv(f"{p}resConfUnit{u}.conv2")
         conv("scratch.output_conv1")
-        conv("scratch.output_conv2.0")
-        conv("scratch.output_conv2.2")
+        if not feature_only:
+            conv("scratch.output_conv2.0")
+            conv("scratch.output_conv2.2")
         self.w = w
         self._graphs, self._emb = GraphCache(), {}
         self.use_cuda_graph = True
@@ -369,19 +389,15 @@ class DPTHeadR3G:
         out = self._fuse("scratch.refinenet2.", out, l2, size=l1.shape[1:3])
         out = self._fuse("scratch.refinenet1.", out, l1)
         out = self._conv3x3("scratch.output_conv1", out)
-        out = ops.bilinear_nhwc(out.contiguous(), ph * self.patch_size, pw * self.patch_size)
+        out = ops.bilinear_nhwc(out.contiguous(), int(ph * self.patch_size / self.down_ratio),
+                                int(pw * self.patch_size / self.down_ratio))
         if self.pos_embed:
             out = out + self._uv(out.shape[-1], out.shape[1], out.shape[2], W, H)
+        if self.feature_only:
+            return out.contiguous()
         out = self._conv3x3("scratch.output_conv2.0", out, act=ops.ACT_RELU)
         fmap = self._conv1x1("scratch.output_conv2.2", out.contiguous(), out_dtype=torch.float32)
-        xyz, conf = fmap[..., :-1], fmap[..., -1]
-        if self.activation == "exp":
-            pts = torch.exp(xyz)
-        elif self.activation == "inv_log":
-            pts = torch.sign(xyz) * torch.expm1(torch.abs(xyz))
-        else:
-            raise ValueError(f"Unknown activation: {self.activation}")
-        return pts, (1 + conf.exp() if self.conf_activation == "expp1" else conf.exp())
+        return _activate(fmap, self.activation, self.conf_activation)
 
     @torch.no_grad()
     def __call__(self, aggregated_tokens_list, images, patch_start_idx, frames_chunk_size=8):
@@ -389,36 +405,116 @@ class DPTHeadR3G:
         toks = [aggregated_tokens_list[layer][:, :, patch_start_idx:].float().reshape(B * S, -1, aggregated_tokens_list[layer].shape[-1]).contiguous()
                 for layer in self.layers]
         if not self.use_cuda_graph:
-            pts, cf = self._impl(toks, H, W)
+            out = self._impl(toks, H, W)
         else:
             g = self._graphs.get((B * S, H, W, toks[0].shape[-1]), toks, lambda *x: self._impl(x, H, W))
             for a, b in zip(g.inputs, toks):
                 a.copy_(b)
             g.replay()
-            pts, cf = (o.clone() for o in g.outputs)
+            out = g.outputs.clone() if self.feature_only else tuple(o.clone() for o in g.outputs)
+        if self.feature_only:
+            return out.view(B, S, *out.shape[1:])
+        pts, cf = out
         return pts.view(B, S, *pts.shape[1:]), cf.view(B, S, *cf.shape[1:])
 
 
+_HEAD_PREFIXES = {"camera": "camera_head.", "depth": "depth_head.", "point": "point_head.", "track": "track_head."}
+
+
 class VGGT:
-    """`model.aggregator / model.camera_head / model.depth_head`, as the stage script uses the reference's VGGT."""
+    """vggt/models/vggt.py on libr3g: `model(images, query_points=None)` returns the reference's predictions dict, and
+    `model.aggregator / model.camera_head / model.depth_head` stay callable one by one, as the stage script uses them.
+
+    enable_camera / enable_depth / enable_point / enable_track: True builds the head (its keys must then be in the
+    state dict), False leaves it out (its predictions are absent), None -- the default -- builds it when the state dict
+    holds its keys.  The keys of a head that is not built are ignored.  On CUDA the heads run on libr3g; on the CPU they
+    are the float32 torch mirrors."""
 
     def __init__(self, img_size=518, patch_size=14, embed_dim=1024, device="cuda", camera_head_kwargs=None,
-                 depth_head_kwargs=None, **agg_kwargs):
+                 depth_head_kwargs=None, point_head_kwargs=None, track_head_kwargs=None, enable_camera=None,
+                 enable_depth=None, enable_point=None, enable_track=None, **agg_kwargs):
         from .vggt import Aggregator
         self.device = torch.device(device)
         self.aggregator = Aggregator(img_size=img_size, patch_size=patch_size, embed_dim=embed_dim, device=device,
                                      **agg_kwargs)
-        self.camera_head = self.depth_head = None
+        self.camera_head = self.depth_head = self.point_head = self.track_head = None
         self.patch_size = patch_size
         self._ck, self._dk = dict(camera_head_kwargs or {}), dict(depth_head_kwargs or {})
+        self._pk, self._tk = dict(point_head_kwargs or {}), dict(track_head_kwargs or {})
+        self._enable = dict(camera=enable_camera, depth=enable_depth, point=enable_point, track=enable_track)
+
+    def _heads_to_build(self, sd, strict):
+        """The heads to build, after checking that each enabled head has keys and (strict) that every key belongs to
+        the aggregator or a head, and those of a built depth / point / track head to its architecture."""
+        build = {}
+        for name, prefix in _HEAD_PREFIXES.items():
+            on = self._enable[name]
+            present = any(k.startswith(prefix) for k in sd)
+            if on and not present:
+                raise KeyError(f"VGGT.load_state_dict: enable_{name}=True but the state dict has no '{prefix}*' keys")
+            build[name] = present if on is None else bool(on)
+        if strict:
+            checked = tuple(_HEAD_PREFIXES[n] for n in ("depth", "point", "track") if build[n])
+            known = set().union(*(_head_keys(n) for n, b in build.items() if b))
+            unexpected = sorted(k for k in sd if not k.startswith(("aggregator.",) + tuple(_HEAD_PREFIXES.values()))
+                                or (k.startswith(checked) and k not in known))
+            if unexpected:
+                raise KeyError(f"VGGT.load_state_dict: unexpected keys {unexpected[:8]}"
+                               + (f" and {len(unexpected) - 8} more" if len(unexpected) > 8 else ""))
+        return build
 
     def load_state_dict(self, sd, strict=True):
+        """Builds the aggregator and the enabled heads from a VGGT state dict (the reference's key names).  A built
+        head whose keys are incomplete raises KeyError naming the missing keys; strict=True also refuses keys that
+        belong to no part of VGGT, or to no layer of a built depth / point / track head."""
+        from .vggt_track import TrackHead, TrackHeadR3G
+        build = self._heads_to_build(sd, strict)
+        need = set().union(*(_head_keys(n) for n, b in build.items() if b))
+        missing = sorted(need - set(sd))
+        if missing:
+            raise KeyError(f"VGGT.load_state_dict: missing keys {missing[:8]}"
+                           + (f" and {len(missing) - 8} more" if len(missing) > 8 else ""))
+        cuda = self.device.type == "cuda"    # the torch mirrors are the CPU side (and the parity tests' other side)
         self.aggregator.load_state_dict(sd, prefix="aggregator.")
-        head = CameraHeadR3G if self.device.type == "cuda" else CameraHead     # the torch mirror is the CPU side (and the parity tests' other side)
-        self.camera_head = head(sd, device=self.device, **self._ck)
-        dpt = DPTHeadR3G if self.device.type == "cuda" else DPTHead
-        self.depth_head = dpt(sd, patch_size=self.patch_size, device=self.device, **self._dk)
+        if build["camera"]:
+            self.camera_head = (CameraHeadR3G if cuda else CameraHead)(sd, device=self.device, **self._ck)
+        dpt = DPTHeadR3G if cuda else DPTHead
+        if build["depth"]:
+            self.depth_head = dpt(sd, patch_size=self.patch_size, device=self.device, **self._dk)
+        if build["point"]:
+            kw = dict(activation="inv_log", conf_activation="expp1", **self._pk)
+            self.point_head = dpt(sd, "point_head.", patch_size=self.patch_size, device=self.device, **kw)
+        if build["track"]:
+            self.track_head = (TrackHeadR3G if cuda else TrackHead)(sd, patch_size=self.patch_size, device=self.device,
+                                                                    **self._tk)
         return self
+
+    @torch.no_grad()
+    def forward(self, images, query_points=None):
+        """images [S, 3, H, W] or [B, S, 3, H, W] in [0, 1]; query_points [N, 2] or [B, N, 2] pixel coordinates.
+        Returns pose_enc [B, S, 9], pose_enc_list, depth [B, S, H, W, 1], depth_conf [B, S, H, W], world_points
+        [B, S, H, W, 3], world_points_conf [B, S, H, W] and images, for the built heads; with query_points and a track
+        head also track [B, S, N, 2] (the last iteration), vis [B, S, N] and conf [B, S, N].  Float32 throughout."""
+        if images.dim() == 4:
+            images = images.unsqueeze(0)
+        if query_points is not None and query_points.dim() == 2:
+            query_points = query_points.unsqueeze(0)
+        tokens, psi = self.aggregator(images)
+        pred = {}
+        if self.camera_head is not None:
+            pose_enc_list = self.camera_head(tokens)
+            pred["pose_enc"], pred["pose_enc_list"] = pose_enc_list[-1], pose_enc_list
+        if self.depth_head is not None:
+            pred["depth"], pred["depth_conf"] = self.depth_head(tokens, images, psi)
+        if self.point_head is not None:
+            pred["world_points"], pred["world_points_conf"] = self.point_head(tokens, images, psi)
+        if self.track_head is not None and query_points is not None:
+            track_list, pred["vis"], pred["conf"] = self.track_head(tokens, images, psi, query_points)
+            pred["track"] = track_list[-1]
+        pred["images"] = images
+        return pred
+
+    __call__ = forward
 
     def eval(self):
         return self
@@ -427,11 +523,99 @@ class VGGT:
         return self
 
 
+def _dpt_state(sd, rn, d, D, features, out_channels, output_dim=2, feature_only=False):
+    """DPTHead's weights (dpt_head.py:53-113) under prefix d, drawn with rn(*shape, s=std)."""
+    sd[d + "norm.weight"], sd[d + "norm.bias"] = torch.ones(D), torch.zeros(D)
+
+    def conv(name, co, ci, k, bias=True, s=None):
+        sd[d + name + ".weight"] = rn(co, ci, k, k, s=s if s is not None else (2.0 / (ci * k * k)) ** 0.5)
+        if bias:
+            sd[d + name + ".bias"] = rn(co)
+    for i, oc in enumerate(out_channels):
+        conv(f"projects.{i}", oc, D, 1)
+        conv(f"scratch.layer{i + 1}_rn", features, oc, 3, bias=False)
+    conv("resize_layers.0", out_channels[0], out_channels[0], 4)     # ConvTranspose2d weight is [in, out, k, k]
+    conv("resize_layers.1", out_channels[1], out_channels[1], 2)
+    conv("resize_layers.3", out_channels[3], out_channels[3], 3)
+    for r in (1, 2, 3, 4):
+        p = f"scratch.refinenet{r}."
+        conv(p + "out_conv", features, features, 1)
+        for u in ((1, 2) if r != 4 else (2,)):
+            conv(f"{p}resConfUnit{u}.conv1", features, features, 3)
+            conv(f"{p}resConfUnit{u}.conv2", features, features, 3)
+    if feature_only:
+        conv("scratch.output_conv1", features, features, 3)
+        return
+    conv("scratch.output_conv1", features // 2, features, 3)
+    conv("scratch.output_conv2.0", 32, features // 2, 3)
+    conv("scratch.output_conv2.2", output_dim, 32, 1, s=0.02)
+
+
+def _tracker_state(sd, rn, t, latent=128, hidden=384, depth=6, corr_levels=7, corr_radius=4, virtual=64):
+    """BaseTrackerPredictor's weights (track_modules/base_track_predictor.py, blocks.py, modules.py) under prefix t."""
+    tdim = 3 * latent + 4
+
+    def lin(name, n, k, s=None):
+        sd[t + name + ".weight"], sd[t + name + ".bias"] = rn(n, k, s=s if s is not None else k ** -0.5), rn(n)
+
+    def norm(name, dim):
+        sd[t + name + ".weight"], sd[t + name + ".bias"] = 1 + rn(dim, s=0.05), rn(dim, s=0.05)
+
+    def block(p, cross):
+        norm(p + "norm1", hidden)
+        if cross:
+            norm(p + "norm_context", hidden)
+        norm(p + "norm2", hidden)
+        a = t + p + ("cross_attn." if cross else "attn.")
+        sd[a + "in_proj_weight"], sd[a + "in_proj_bias"] = rn(3 * hidden, hidden, s=hidden ** -0.5), rn(3 * hidden)
+        sd[a + "out_proj.weight"], sd[a + "out_proj.bias"] = rn(hidden, hidden, s=hidden ** -0.5 / 2), rn(hidden)
+        lin(p + "mlp.fc1", 4 * hidden, hidden)
+        lin(p + "mlp.fc2", hidden, 4 * hidden, s=(4 * hidden) ** -0.5 / 2)
+    lin("corr_mlp.fc1", hidden, corr_levels * (2 * corr_radius + 1) ** 2)
+    lin("corr_mlp.fc2", latent, hidden)
+    sd[t + "query_ref_token"] = rn(1, 2, tdim, s=0.1)
+    u = "updateformer."
+    norm(u + "input_norm", tdim)
+    lin(u + "input_transform", hidden, tdim)
+    norm(u + "output_norm", hidden)
+    lin(u + "flow_head", latent + 2, hidden, s=0.004)
+    sd[t + u + "virual_tracks"] = rn(1, virtual, 1, hidden, s=1.0)
+    for i in range(depth):
+        block(f"{u}time_blocks.{i}.", False)
+    for i in range(depth):
+        block(f"{u}space_virtual_blocks.{i}.", False)
+    for i in range(depth):
+        block(f"{u}space_point2virtual_blocks.{i}.", True)
+    for i in range(depth):
+        block(f"{u}space_virtual2point_blocks.{i}.", True)
+    norm("fmap_norm", latent)
+    norm("ffeat_norm", latent)
+    lin("ffeat_updater.0", latent, latent)
+    lin("vis_predictor.0", 1, latent)
+    lin("conf_predictor.0", 1, latent)
+
+
+def _head_keys(name):
+    """The state-dict keys of one VGGT head (without the camera head, whose trunk depth is a constructor argument)."""
+    sd = {}
+    meta = lambda *shape, s=None: torch.empty(shape, device="meta")  # noqa: E731
+    if name in ("depth", "point"):
+        _dpt_state(sd, meta, _HEAD_PREFIXES[name], 1, 2, (1, 1, 1, 1))
+    elif name == "track":
+        _dpt_state(sd, meta, "track_head.feature_extractor.", 1, 2, (1, 1, 1, 1), feature_only=True)
+        _tracker_state(sd, meta, "track_head.tracker.")
+    return set(sd)
+
+
 def random_state_dict(seed=0, embed_dim=1024, depth=24, vit_depth=24, trunk_depth=4, features=256,
-                      out_channels=(256, 512, 1024, 1024), patch_size=14, img_size=518, std=0.02):
-    """Seeded random weights with the key names and shapes of VGGT-1B's camera + depth model (SURVEY.md Appendix C;
-    vggt/models/vggt.py, aggregator.py:71-120, camera_head.py:28-70, dpt_head.py:53-113).  No checkpoint is reachable
-    from this build environment, so bench.py's config-4 workload and the GPU tests run on these."""
+                      out_channels=(256, 512, 1024, 1024), patch_size=14, img_size=518, std=0.02, full=False,
+                      patch_embed="dinov2"):
+    """Seeded random weights with the key names and shapes of VGGT-1B (SURVEY.md Appendix C; vggt/models/vggt.py,
+    aggregator.py:71-120, camera_head.py:28-70, dpt_head.py:53-113): the camera + depth model, and with full=True also
+    the point head (dpt_head.py, output_dim 4) and the track head (track_head.py: a 128-feature DPT extractor and the
+    tracker), drawn after the others so that the camera + depth weights of a seed do not depend on `full`.
+    patch_embed="conv" gives the aggregator a convolutional patch embedding instead of the DINOv2 one.  No checkpoint is
+    reachable from this build environment, so bench.py's config-4 workload and the GPU tests run on these."""
     g = torch.Generator().manual_seed(seed)
     C = embed_dim
     sd = {}
@@ -453,13 +637,16 @@ def random_state_dict(seed=0, embed_dim=1024, depth=24, vit_depth=24, trunk_dept
     a = "aggregator."
     sd[a + "camera_token"], sd[a + "register_token"] = rn(1, 2, 1, C), rn(1, 2, 4, C)
     pe = a + "patch_embed."
-    sd[pe + "patch_embed.proj.weight"], sd[pe + "patch_embed.proj.bias"] = rn(C, 3, patch_size, patch_size), torch.zeros(C)
-    sd[pe + "cls_token"], sd[pe + "register_tokens"] = rn(1, 1, C), rn(1, 4, C)
-    sd[pe + "pos_embed"] = rn(1, 1 + (img_size // patch_size) ** 2, C)
-    sd[pe + "mask_token"] = torch.zeros(1, C)
-    sd[pe + "norm.weight"], sd[pe + "norm.bias"] = torch.ones(C), torch.zeros(C)
-    for i in range(vit_depth):
-        block(f"{pe}blocks.{i}.", C, False)
+    if patch_embed == "conv":
+        sd[pe + "proj.weight"], sd[pe + "proj.bias"] = rn(C, 3, patch_size, patch_size), torch.zeros(C)
+    else:
+        sd[pe + "patch_embed.proj.weight"], sd[pe + "patch_embed.proj.bias"] = rn(C, 3, patch_size, patch_size), torch.zeros(C)
+        sd[pe + "cls_token"], sd[pe + "register_tokens"] = rn(1, 1, C), rn(1, 4, C)
+        sd[pe + "pos_embed"] = rn(1, 1 + (img_size // patch_size) ** 2, C)
+        sd[pe + "mask_token"] = torch.zeros(1, C)
+        sd[pe + "norm.weight"], sd[pe + "norm.bias"] = torch.ones(C), torch.zeros(C)
+        for i in range(vit_depth):
+            block(f"{pe}blocks.{i}.", C, False)
     for i in range(depth):
         block(f"{a}frame_blocks.{i}.", C, True)
         block(f"{a}global_blocks.{i}.", C, True)
@@ -477,26 +664,9 @@ def random_state_dict(seed=0, embed_dim=1024, depth=24, vit_depth=24, trunk_dept
     for i in range(trunk_depth):
         block(f"{c}trunk.{i}.", D, False)
         sd[f"{c}trunk.{i}.ls1.gamma"], sd[f"{c}trunk.{i}.ls2.gamma"] = torch.full((D,), 0.01), torch.full((D,), 0.01)
-    d = "depth_head."
-    sd[d + "norm.weight"], sd[d + "norm.bias"] = torch.ones(D), torch.zeros(D)
-
-    def conv(name, co, ci, k, bias=True, s=None):
-        sd[d + name + ".weight"] = rn(co, ci, k, k, s=s if s is not None else (2.0 / (ci * k * k)) ** 0.5)
-        if bias:
-            sd[d + name + ".bias"] = rn(co)
-    for i, oc in enumerate(out_channels):
-        conv(f"projects.{i}", oc, D, 1)
-        conv(f"scratch.layer{i + 1}_rn", features, oc, 3, bias=False)
-    conv("resize_layers.0", out_channels[0], out_channels[0], 4)     # ConvTranspose2d weight is [in, out, k, k]
-    conv("resize_layers.1", out_channels[1], out_channels[1], 2)
-    conv("resize_layers.3", out_channels[3], out_channels[3], 3)
-    for r in (1, 2, 3, 4):
-        p = f"scratch.refinenet{r}."
-        conv(p + "out_conv", features, features, 1)
-        for u in ((1, 2) if r != 4 else (2,)):
-            conv(f"{p}resConfUnit{u}.conv1", features, features, 3)
-            conv(f"{p}resConfUnit{u}.conv2", features, features, 3)
-    conv("scratch.output_conv1", features // 2, features, 3)
-    conv("scratch.output_conv2.0", 32, features // 2, 3)
-    conv("scratch.output_conv2.2", 2, 32, 1, s=0.02)
+    _dpt_state(sd, rn, "depth_head.", D, features, out_channels)
+    if full:
+        _dpt_state(sd, rn, "point_head.", D, features, out_channels, output_dim=4)
+        _dpt_state(sd, rn, "track_head.feature_extractor.", D, 128, (256, 512, 1024, 1024), feature_only=True)
+        _tracker_state(sd, rn, "track_head.tracker.")
     return sd
