@@ -356,6 +356,81 @@ __device__ __forceinline__ void wgmma_tile(float* acc, uint64_t da, uint64_t db)
   else wgmma_m64n128k16_ss(acc, da, db, 1u);
 }
 
+// The operand ring, shared by linear_kernel and moe_gemm_kernel so that a row's accumulators are the same in both:
+// Cfg<BN>::kStages slots of one BM x BK tile of X and one BN x BK tile of W at the 1024-aligned smem, followed by the
+// slots' full / empty barriers.  ring_init (one thread) runs before the __syncthreads that publishes the barriers.
+template <int BN>
+__device__ __forceinline__ void ring_init(const CUtensorMap* tmap_x, const CUtensorMap* tmap_w, uint64_t* full_bar,
+                                          uint64_t* empty_bar) {
+  tma_prefetch_desc(tmap_x);
+  tma_prefetch_desc(tmap_w);
+  for (int s = 0; s < Cfg<BN>::kStages; ++s) {
+    mbar_init(&full_bar[s], 1);
+    mbar_init(&empty_bar[s], 32 * kNumEpilogueWarps);   // every consumer thread releases the slot
+  }
+  fence_barrier_init();
+}
+
+// TMA producer (one thread): every k-block of the tile's X rows [x_row, x_row + BM) of segment x_seg and W rows
+// [w_row, w_row + BN), each into the next free slot
+template <int BN>
+__device__ __forceinline__ void ring_produce(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                             const CUtensorMap* tmap_x, const CUtensorMap* tmap_w, int x_row,
+                                             int x_seg, int w_row, int num_k_blocks) {
+  using C = Cfg<BN>;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < num_k_blocks; ++kb) {
+    mbar_wait(&empty_bar[stage], phase ^ 1);
+    uint8_t* sa = smem + stage * C::kStageBytes;
+    uint8_t* sb = sa + C::kStageBytesA;
+    mbar_expect_tx(&full_bar[stage], C::kStageBytes);
+    tma_load_3d(sa, tmap_x, &full_bar[stage], kb * BK, x_row, x_seg, kEvictFirst);
+    tma_load_2d(sb, tmap_w, &full_bar[stage], kb * BK, w_row, kEvictLast);
+    if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+  }
+}
+
+// Consumers (warps 0..7, warpgroup g: MMA rows [64 g, 64 g + 64)): the main loop over the ring, then the fp32
+// accumulator tile staged row-major (Cfg<BN>::kLdStage floats per row) over the ring, visible to all 256 threads
+template <int BN>
+__device__ __forceinline__ void ring_consume(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                             int num_k_blocks, int warp, int lane) {
+  using C = Cfg<BN>;
+  const int wg = warp >> 2;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0, prev = 0;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < num_k_blocks; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + stage * C::kStageBytes) + wg * 64 * 128;
+    const uint32_t sb = smem_u32(smem + stage * C::kStageBytes + C::kStageBytesA);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+      wgmma_tile<BN>(acc, gmma_desc_sw128(sa + k * 32, 1024, 16), gmma_desc_sw128(sb + k * 32, 1024, 16));
+    wgmma_commit();
+    wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot goes back to the producer
+    if (kb > 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == C::kStages) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_reg_fence<BN / 2>(acc);
+  named_bar_sync(1, 32 * kNumEpilogueWarps);   // both warpgroups are done reading the ring
+  float* acc_smem = reinterpret_cast<float*>(smem);
+  const int w4 = warp & 3;
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 2) {
+    const int row = wg * 64 + w4 * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+    const int col = 8 * (i >> 2) + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(acc_smem + row * C::kLdStage + col) = make_float2(acc[i], acc[i + 1]);
+  }
+  named_bar_sync(1, 32 * kNumEpilogueWarps);
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kNumThreads, Cfg<BN>::kMinBlocks)
 linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant__ CUtensorMap tmap_w0,
@@ -386,42 +461,21 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
   const int tm = lt / p.tiles_n, tn = lt % p.tiles_n;
   const int sg = tm / p.tiles_per_seg;
   const int num_k_blocks = (p.K + BK - 1) / BK;
+  const CUtensorMap* tmap_x = which == 2 ? &tmap_x2 : which == 1 ? &tmap_x1 : &tmap_x0;
+  const CUtensorMap* tmap_w = which == 2 ? &tmap_w2 : which == 1 ? &tmap_w1 : &tmap_w0;
 
-  if (warp == kNumEpilogueWarps && lane == 0) {
-    tma_prefetch_desc(which == 2 ? &tmap_x2 : which == 1 ? &tmap_x1 : &tmap_x0);
-    tma_prefetch_desc(which == 2 ? &tmap_w2 : which == 1 ? &tmap_w1 : &tmap_w0);
-    for (int s = 0; s < C::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 32 * kNumEpilogueWarps);   // every consumer thread releases the slot
-    }
-    fence_barrier_init();
-  }
+  if (warp == kNumEpilogueWarps && lane == 0) ring_init<BN>(tmap_x, tmap_w, full_bar, empty_bar);
   __syncthreads();
   pdl_wait();   // everything above overlapped the previous kernel's tail; its results are visible from here on
 
   if (warp == kNumEpilogueWarps) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      const CUtensorMap* tmap_x = which == 2 ? &tmap_x2 : which == 1 ? &tmap_x1 : &tmap_x0;
-      const CUtensorMap* tmap_w = which == 2 ? &tmap_w2 : which == 1 ? &tmap_w1 : &tmap_w0;
-      const int l0 = (tm % p.tiles_per_seg) * BM;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_k_blocks; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * C::kStageBytes;
-        uint8_t* sb = sa + C::kStageBytesA;
-        mbar_expect_tx(&full_bar[stage], C::kStageBytes);
-        tma_load_3d(sa, tmap_x, &full_bar[stage], kb * BK, l0, sg, kEvictFirst);
-        tma_load_2d(sb, tmap_w, &full_bar[stage], kb * BK, tn * BN, kEvictLast);
-        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-      }
-    }
+    if (lane == 0)
+      ring_produce<BN>(smem, full_bar, empty_bar, tmap_x, tmap_w, (tm % p.tiles_per_seg) * BM, sg, tn * BN,
+                       num_k_blocks);
     return;
   }
 
   // -------------------------------------------------------------------- consumers (warps 0..7)
-  const int wg = warp >> 2;                     // warpgroup: MMA rows [64 wg, 64 wg + 64)
   uint4* wsm = reinterpret_cast<uint4*>(epi_smem + warp * kEpiSmemPerWarp);
   // stage the warp's bias / gate slices before the main loop: the loads land while the tensor cores work.  The
   // row-derived epilogue values are recomputed after the loop instead of being held in registers across it.
@@ -435,38 +489,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tmap_x0, const __grid_constant
                                  sg * p.seg_len + l31, l < p.seg_len ? sg * p.seg_len + l : sg * p.seg_len + l31);
   }
 
-  {
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0, prev = 0;
-    uint32_t phase = 0;
-    for (int kb = 0; kb < num_k_blocks; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * C::kStageBytes) + wg * 64 * 128;
-      const uint32_t sb = smem_u32(smem + stage * C::kStageBytes + C::kStageBytesA);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k)
-        wgmma_tile<BN>(acc, gmma_desc_sw128(sa + k * 32, 1024, 16), gmma_desc_sw128(sb + k * 32, 1024, 16));
-      wgmma_commit();
-      wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot goes back to the producer
-      if (kb > 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    wgmma_reg_fence<BN / 2>(acc);
-    named_bar_sync(1, 32 * kNumEpilogueWarps);   // both warpgroups are done reading the ring
-    const int w4 = warp & 3;
-#pragma unroll
-    for (int i = 0; i < BN / 2; i += 2) {
-      const int row = wg * 64 + w4 * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-      const int col = 8 * (i >> 2) + 2 * (lane & 3);
-      *reinterpret_cast<float2*>(acc_smem + row * C::kLdStage + col) = make_float2(acc[i], acc[i + 1]);
-    }
-    named_bar_sync(1, 32 * kNumEpilogueWarps);
-  }
+  ring_consume<BN>(smem, full_bar, empty_bar, num_k_blocks, warp, lane);
 
   // -------------------------------------------------------------------- epilogue: one row, half of the columns
   const int row_in_tile = threadIdx.x & (BM - 1);   // epilogue row
@@ -516,26 +539,32 @@ struct Problem {
   CUtensorMap tx, tw;
 };
 
+// The ring's operand maps (ring_produce): X as nseg segments of seg_len rows of K halfs (row stride ldx, segment stride
+// seg_stride rows), read as BM x BK boxes; W as w_rows rows of K halfs, read as box_n x BK boxes.
+int make_operand_maps(r3g_ctx* ctx, const void* x, int64_t ldx, int64_t seg_len, int nseg, int64_t seg_stride,
+                      const void* w, int64_t w_rows, int K, int box_n, CUtensorMap& tx, CUtensorMap& tw) {
+  {
+    const uint64_t dims[3] = {(uint64_t)K, (uint64_t)seg_len, (uint64_t)nseg};
+    const uint64_t strides[3] = {2, (uint64_t)ldx * 2, (uint64_t)seg_stride * ldx * 2};
+    const uint32_t box[3] = {BK, BM, 1};
+    int rc = r3g_make_tmap_f16(ctx, &tx, x, 3, dims, strides, box);
+    if (rc) return rc;
+  }
+  const uint64_t dims[2] = {(uint64_t)K, (uint64_t)w_rows};
+  const uint64_t strides[2] = {2, (uint64_t)K * 2};
+  const uint32_t box[2] = {BK, (uint32_t)box_n};
+  return r3g_make_tmap_f16(ctx, &tw, w, 2, dims, strides, box);
+}
+
 int make_problem(r3g_ctx* ctx, const r3g_linear_args* a, int tile_m, int box_n, int bn, Problem& out) {
   LinearParams& p = out.p;
   memset(&p, 0, sizeof(p));
   if (!a) return R3G_OK;   // no such problem: tiles_m = 0
   const int seg_len = a->seg_len > 0 ? a->seg_len : a->M;
   const int nseg = a->M / seg_len;
-  {
-    const uint64_t dims[3] = {(uint64_t)a->K, (uint64_t)seg_len, (uint64_t)nseg};
-    const uint64_t strides[3] = {2, (uint64_t)a->ldx * 2, (uint64_t)(nseg > 1 ? a->x_seg_stride : seg_len) * a->ldx * 2};
-    const uint32_t box[3] = {BK, BM, 1};
-    int rc = r3g_make_tmap_f16(ctx, &out.tx, a->x, 3, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->N};
-    const uint64_t strides[2] = {2, (uint64_t)a->K * 2};
-    const uint32_t box[2] = {BK, (uint32_t)box_n};
-    int rc = r3g_make_tmap_f16(ctx, &out.tw, a->w, 2, dims, strides, box);
-    if (rc) return rc;
-  }
+  int rc = make_operand_maps(ctx, a->x, a->ldx, seg_len, nseg, nseg > 1 ? a->x_seg_stride : seg_len, a->w, a->N, a->K,
+                             box_n, out.tx, out.tw);
+  if (rc) return rc;
   p.M = a->M; p.N = a->N; p.K = a->K;
   p.bias = (const __half*)a->bias;
   p.y = a->y; p.ldy = a->ldy;
@@ -679,9 +708,10 @@ moe_route_kernel(const __half* __restrict__ x, int64_t ldx, const __half* __rest
   }
 }
 
-// Grouped expert GEMM (moe_mode 2) and the shared expert's combine GEMM (moe_mode 3): linear_kernel<128>'s producer,
-// main loop and accumulator staging, so that a row's accumulators are those r3g_linear computes for it, with a per-row
-// epilogue in which each thread writes its own row.  No PDL: the row counts come from the route launch before it.
+// Grouped expert GEMM (moe_mode 2) and the shared expert's combine GEMM (moe_mode 3): the operand ring of
+// linear_kernel<128> (ring_init / ring_produce / ring_consume; X as one segment of groups * M rows), so that a row's
+// accumulators are those r3g_linear computes for it, with a per-row epilogue in which each thread writes its own row.
+// No PDL: the row counts come from the route launch before it.
 struct MoeParams {
   int M, N, K;               // M: rows per group (grouped) or rows (combine)
   int groups, experts, tiles_m, tiles_n;
@@ -718,66 +748,16 @@ moe_gemm_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   const int num_k_blocks = (p.K + BK - 1) / BK;
   const int row0 = g * p.M + tm * BM;   // first x / y row of the tile
 
-  if (warp == kNumEpilogueWarps && lane == 0) {
-    tma_prefetch_desc(&tmap_x);
-    tma_prefetch_desc(&tmap_w);
-    for (int s = 0; s < C::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 32 * kNumEpilogueWarps);
-    }
-    fence_barrier_init();
-  }
+  if (warp == kNumEpilogueWarps && lane == 0) ring_init<BN>(&tmap_x, &tmap_w, full_bar, empty_bar);
   __syncthreads();
 
   if (warp == kNumEpilogueWarps) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_k_blocks; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * C::kStageBytes;
-        mbar_expect_tx(&full_bar[stage], C::kStageBytes);
-        tma_load_2d(sa, &tmap_x, &full_bar[stage], kb * BK, row0, kEvictFirst);
-        tma_load_2d(sa + C::kStageBytesA, &tmap_w, &full_bar[stage], kb * BK, g * p.N + tn * BN, kEvictLast);
-        if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-      }
-    }
+    if (lane == 0)
+      ring_produce<BN>(smem, full_bar, empty_bar, &tmap_x, &tmap_w, row0, 0, g * p.N + tn * BN, num_k_blocks);
     return;
   }
 
-  const int wg = warp >> 2;
-  {
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0, prev = 0;
-    uint32_t phase = 0;
-    for (int kb = 0; kb < num_k_blocks; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * C::kStageBytes) + wg * 64 * 128;
-      const uint32_t sb = smem_u32(smem + stage * C::kStageBytes + C::kStageBytesA);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k)
-        wgmma_tile<BN>(acc, gmma_desc_sw128(sa + k * 32, 1024, 16), gmma_desc_sw128(sb + k * 32, 1024, 16));
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (kb > 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == C::kStages) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    wgmma_reg_fence<BN / 2>(acc);
-    named_bar_sync(1, 32 * kNumEpilogueWarps);
-    const int w4 = warp & 3;
-#pragma unroll
-    for (int i = 0; i < BN / 2; i += 2) {
-      const int row = wg * 64 + w4 * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-      const int col = 8 * (i >> 2) + 2 * (lane & 3);
-      *reinterpret_cast<float2*>(acc_smem + row * C::kLdStage + col) = make_float2(acc[i], acc[i + 1]);
-    }
-    named_bar_sync(1, 32 * kNumEpilogueWarps);
-  }
+  ring_consume<BN>(smem, full_bar, empty_bar, num_k_blocks, warp, lane);
 
   // epilogue: one row, half of the tile's columns, 8 columns at a time
   const int row_in_tile = threadIdx.x & (BM - 1);
@@ -863,22 +843,10 @@ int launch_moe_gemm(r3g_ctx* ctx, const r3g_linear_args* a, cudaStream_t s) {
               : (a->moe_experts < 0 || a->moe_experts > groups || a->moe_cap != a->M ||
                  (a->moe_experts && !a->moe_counts) || a->residual || a->moe_slot_y))
     return r3g_fail(ctx, R3G_E_INVALID, "linear (moe %s): inconsistent moe operands", combine ? "combine" : "grouped");
-  Problem pr;
-  memset(&pr, 0, sizeof(pr));
-  {
-    const uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)groups * a->M};
-    const uint64_t strides[2] = {2, (uint64_t)a->ldx * 2};
-    const uint32_t box[2] = {BK, BM};
-    int rc = r3g_make_tmap_f16(ctx, &pr.tx, a->x, 2, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)groups * a->N};
-    const uint64_t strides[2] = {2, (uint64_t)a->K * 2};
-    const uint32_t box[2] = {BK, 128};
-    int rc = r3g_make_tmap_f16(ctx, &pr.tw, a->w, 2, dims, strides, box);
-    if (rc) return rc;
-  }
+  CUtensorMap tx, tw;
+  const int64_t rows = (int64_t)groups * a->M;
+  int rc = make_operand_maps(ctx, a->x, a->ldx, rows, 1, rows, a->w, (int64_t)groups * a->N, a->K, 128, tx, tw);
+  if (rc) return rc;
   MoeParams p;
   memset(&p, 0, sizeof(p));
   p.M = a->M; p.N = a->N; p.K = a->K;
@@ -903,7 +871,7 @@ int launch_moe_gemm(r3g_ctx* ctx, const r3g_linear_args* a, cudaStream_t s) {
     R3G_CUDA_OK(ctx, cudaFuncSetAttribute(moe_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     ctx->attr_done |= R3G_ATTR_MOE_GEMM;
   }
-  moe_gemm_kernel<<<(unsigned)(groups * p.tiles_m * p.tiles_n), kNumThreads, C::kSmemBytes, s>>>(pr.tx, pr.tw, p);
+  moe_gemm_kernel<<<(unsigned)(groups * p.tiles_m * p.tiles_n), kNumThreads, C::kSmemBytes, s>>>(tx, tw, p);
   R3G_LAUNCH_OK(ctx);
   return R3G_OK;
 }

@@ -2,7 +2,8 @@
 every output element's k16 accumulation order and its epilogue arithmetic, so the outputs of the cases below must hash
 to the digests in tests/golden/gemm_persistent.json, recorded with tools/make_gemm_golden.py from the one-tile-per-CTA
 kernel of gemm.cu.  The cases cover the bounds shapes, every epilogue, grouped launches, segmented A, one k-block, K not
-a multiple of 64, fewer tiles than SMs and 2 * 132 + 1 tiles (H100 SXM)."""
+a multiple of 64, fewer tiles than SMs and 2 * 132 + 1 tiles (H100 SXM), and the MoE grouped and combine modes, whose
+kernel shares linear_kernel's operand ring."""
 
 import hashlib
 import json
@@ -99,6 +100,32 @@ def _group(ops, n):
     return list(ops.linear_group(*probs))
 
 
+def _moe_grouped(ops, act, scaled, G=5, cap=300, N=392, K=1000, seed=51):
+    """4 routed experts with a full-capacity, an empty, a 129-row (partial last tile) and a 5-row segment, and a last
+    group of cap rows; N = 392 ends in a partial column tile.  Rows past a segment's count keep out's initial values."""
+    x, b = _randn(G * cap, K, seed=seed), _randn(G, N, seed=seed + 1)
+    w = _randn(G, N, K, std=K ** -0.5, seed=seed + 2)
+    counts = torch.tensor([cap, 0, 129, 5], dtype=torch.int32, device=DEV)
+    out = _randn(G * cap, N, seed=seed + 3)
+    rs = _randn(G * cap, std=0.2, mean=0.5, seed=seed + 4) if scaled else None
+    return ops.moe_grouped(x, w, b, counts=counts, experts=4, out=out, act=act, row_scale=rs)
+
+
+def _moe_combine(ops, M=1000, N=256, K=512, E=4, seed=61):
+    """The shared expert's fc2 + the top-2 expert sum + the residual, in place; each row's two experts are distinct and
+    in either order."""
+    x, w, b = _inputs(M, N, K, seed)
+    g = torch.Generator().manual_seed(seed + 3)
+    e0 = torch.randint(0, E, (M,), generator=g)
+    e1 = (e0 + torch.randint(1, E, (M,), generator=g)) % E
+    ids = torch.stack([e0, e1], 1)
+    slots = ids * M + torch.arange(M)[:, None]
+    out = _randn(M, N, seed=seed + 4)
+    ops.moe_combine(x, w, b, slot_y=_randn(E * M, N, std=0.5, seed=seed + 5), ids=ids.int().to(DEV),
+                    slots=slots.int().to(DEV), residual=out, out=out)
+    return out
+
+
 def cases():
     """{name: zero-argument callable returning the output tensor(s)} of every case."""
     from r3g import ops
@@ -124,6 +151,12 @@ def cases():
                     (265 * 128, 128, 192), (133 * 128, 256, 320), (132 * 128, 256, 1024), (8884, 7168, 1024)]:
         c[f"tiles_{M}x{N}x{K}_gelu_erf"] = lambda M=M, N=N, K=K: ops.linear(
             *_inputs(M, N, K, seed=M + N + K), act=ops.ACT_GELU_ERF)
+    # the MoE modes (moe_gemm_kernel): grouped with and without erf-GELU and the row scale, and combine
+    for act in ("none", "gelu_erf"):
+        for scaled in (False, True):
+            c[f"moe_grouped_{act}{'_scaled' if scaled else ''}"] = lambda act=act, scaled=scaled: _moe_grouped(
+                ops, ops.ACT_GELU_ERF if act == "gelu_erf" else ops.ACT_NONE, scaled)
+    c["moe_combine_top2"] = lambda: _moe_combine(ops)
     return c
 
 

@@ -41,7 +41,8 @@ def _one(funcs, *needles):
 def test_gemm_is_wgmma_tma_and_has_no_gpu_scope_membar(sass):
     funcs, usage = sass
     for name, shape in ((_one(funcs, "linear_kernelILi128E")[0], "64x128x16"),
-                        (_one(funcs, "linear_kernelILi256E")[0], "64x256x16")):
+                        (_one(funcs, "linear_kernelILi256E")[0], "64x256x16"),
+                        (_one(funcs, "moe_gemm_kernel")[0], "64x128x16")):
         body = funcs[name]
         assert "HGMMA." + shape + ".F32" in body and "UTMALDG" in body, name
         assert "MEMBAR.ALL.GPU" not in body, name + ": a GPU-scope membar in the pipeline"

@@ -1,10 +1,12 @@
 #!/usr/bin/env python
-"""Time r3g_linear at every GEMM shape of one DiT forward and one decode chunk, with its real epilogue: CUDA events
-around replays of a CUDA graph of `--reps` launches, after a warm-up.  Prints one JSON line per shape (ms per launch,
-executed TFLOP/s = 2 M N K / time).  --tree times the library of another tree (e.g. the parent commit extracted into
-ab_parent/ and built there), so two arms can be compared in one session:
+"""Time r3g_linear at every GEMM shape of one DiT forward and one decode chunk, with its real epilogue, and the grouped
+fc1, grouped fc2 and combine launches of one Hunyuan3D-2mini MoE layer: CUDA events around replays of a CUDA graph of
+`--reps` launches, after a warm-up.  Prints one JSON line per shape (ms per launch, executed TFLOP/s = 2 M N K / time,
+M = the rows computed).  --tree times the library of another tree (e.g. the parent commit extracted into ab_parent/ and
+built there), so two arms can be compared in one session:
   python tools/ab_gemm.py --tree ab_parent; python tools/ab_gemm.py"""
 import argparse
+import itertools
 import json
 import os
 import sys
@@ -37,6 +39,42 @@ def shapes(ops):
     ]
 
 
+def linear_launches(ops):
+    """(name, M, N, K, launch) of shapes(), each on fresh random operands."""
+    for name, M, N, K, kw in shapes(ops):
+        x = torch.randn(M, K, device="cuda").half()
+        w = (torch.randn(N, K, device="cuda") * K ** -0.5).half()
+        b = torch.randn(N, device="cuda").half()
+        y = torch.randn(M, N, device="cuda").half()
+        if kw.pop("residual", False):
+            kw["residual"] = y
+        yield name, M, N, K, lambda: ops.linear(x, w, b, out=y, **kw)
+
+
+def moe_launches(ops):
+    """(name, rows, N, K, launch) of the three GEMMs of one 2mini MoE layer (HunYuanDiTPlain._moe) on a CFG pair: M = 2 x
+    (512 latents + 1) rows routed top-2 over 8 experts by a random gate; fc1 computes the experts' 2 M rows and the shared
+    expert's M, fc2 the experts' 2 M, combine the shared expert's M."""
+    from r3g.pipelines import HUNYUAN3D_2MINI_CONFIG
+    cfg = HUNYUAN3D_2MINI_CONFIG["model"]
+    H, E, k = cfg["hidden_size"], cfg["num_experts"], cfg["moe_top_k"]
+    M = 2 * (HUNYUAN3D_2MINI_CONFIG["vae"]["num_latents"] + 1)
+    f16 = lambda *s, std=1.0: (torch.randn(*s, device="cuda") * std).half()  # noqa: E731
+    i32 = lambda *s: torch.empty(*s, device="cuda", dtype=torch.int32)  # noqa: E731
+    SX, SH, SY = f16((E + 1) * M, H), f16((E + 1) * M, 4 * H), f16(E * M, H)
+    r = dict(slot_scale=f16(E * M), counts=i32(E), ids=i32(M, k), weights=f16(M, k), slots=i32(M, k))
+    ops.moe_route(SX[E * M:], f16(E, H, std=H ** -0.5), top_k=k, cap=M, slot_x=SX, **r)
+    w1, b1 = f16(E + 1, 4 * H, H, std=H ** -0.5), f16(E + 1, 4 * H)
+    w2, b2 = f16(E, H, 4 * H, std=(4 * H) ** -0.5), f16(E, H)
+    wc, bc, s = f16(H, 4 * H, std=(4 * H) ** -0.5), f16(H), f16(M, H)
+    yield "mini.moe.fc1", (k + 1) * M, 4 * H, H, lambda: ops.moe_grouped(
+        SX, w1, b1, counts=r["counts"], experts=E, out=SH, act=ops.ACT_GELU_ERF)
+    yield "mini.moe.fc2", k * M, H, 4 * H, lambda: ops.moe_grouped(
+        SH[:E * M], w2, b2, counts=r["counts"], experts=E, out=SY, row_scale=r["slot_scale"])
+    yield "mini.moe.combine", M, H, 4 * H, lambda: ops.moe_combine(
+        SH[E * M:], wc, bc, slot_y=SY, ids=r["ids"], slots=r["slots"], residual=s, out=s)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--tree", default=ROOT, help="repository tree whose built libr3g is timed")
@@ -47,21 +85,15 @@ def main():
     from r3g import ops
     torch.manual_seed(0)
     arm = os.path.relpath(os.path.abspath(args.tree), ROOT)
-    for name, M, N, K, kw in shapes(ops):
-        x = torch.randn(M, K, device="cuda").half()
-        w = (torch.randn(N, K, device="cuda") * K ** -0.5).half()
-        b = torch.randn(N, device="cuda").half()
-        y = torch.randn(M, N, device="cuda").half()
-        if kw.pop("residual", False):
-            kw["residual"] = y
+    for name, M, N, K, launch in itertools.chain(linear_launches(ops), moe_launches(ops)):
         for _ in range(3):
-            ops.linear(x, w, b, out=y, **kw)
+            launch()
         torch.cuda.synchronize()
         s = torch.cuda.Stream()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.stream(s), torch.cuda.graph(g, stream=s):
             for _ in range(args.reps):
-                ops.linear(x, w, b, out=y, **kw)
+                launch()
         g.replay()
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
