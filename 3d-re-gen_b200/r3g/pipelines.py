@@ -431,67 +431,74 @@ class Hunyuan3DDiTPipeline:
 
 class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
 
-    def _denoise(self, latents, cond, timesteps, guidance_scale, callback=None, callback_steps=None, object_group=None):
+    def _schedule(self, timesteps):
+        """(t16, dsig) of `timesteps`.  t16: the model's timesteps, t.to(fp16) / num_train_timesteps evaluated in fp16
+        as the reference does.  dsig[i]: sigma[i + 1] - sigma[i] rounded to fp16, because torch multiplies the fp16
+        model output by the 0-dim fp32 (sigma_next - sigma) after casting it to the result dtype (schedulers.py:305)."""
+        sig = self.scheduler.step_sigmas()
+        t16 = (timesteps.to(torch.float16) / self.scheduler.config.num_train_timesteps).to(self.device)
+        return t16, [float((sig[i + 1] - sig[i]).to(torch.float16)) for i in range(len(timesteps))]
+
+    def _dit_step(self, x, ctx, shared, guidance_scale):
+        """The DiT forward of one denoising step on the model input x [b, Li, C] and the context ctx [b, Lt, D].
+        Returns (x_in, t_buf, step): the loop writes each step's timesteps into t_buf and may update x_in in place, and
+        step() runs the forward on them and returns v.  With CUDA graphs on (and no taps to record), x_in and t_buf
+        are static inputs of the graph for (x shape, ctx shape, shared), loaded with x, and step() is one replay.
+
+        A guidance-distilled model also reads [guidance_scale] * b in fp16 (pipelines.py:733-737).  A model with
+        project_context reads every block's cross-attention k / v of the context; they are the same at every step, so
+        they are projected once per call, outside the step graph, into the buffer the step reads: a cached graph's
+        static input, or else a new tensor that a capture copies into its own.  `shared` (the unconditional sample's
+        text rows are all one vector, see Hunyuan3DDiT.forward's uncond_txt_shared) depends on this call's context, so
+        the collapsed branch is chosen per call: `shared` is part of the graph key."""
+        model, b = self.model, x.shape[0]
+        t_buf = torch.full((b,), 0.5, device=self.device, dtype=torch.float16)  # warm-up t; set per step
+        kw = {}
+        if _guidance_distilled(model):
+            kw["guidance"] = torch.tensor([guidance_scale] * b, dtype=torch.float16).to(self.device)
+        graphed = self.use_cuda_graph and model.taps is None
+        key = (x.shape, ctx.shape, shared)
+        cached = self._graphs.entries.get(key) if graphed else None
+        proj = _context_kv(model)
+        if proj is not None:
+            kw["context_kv"] = proj(ctx, out=None if cached is None else cached.inputs[-1])
+
+        def forward(xs, ts, cs, *rest):
+            return model(xs, ts, {"main": cs}, uncond_txt_shared=shared, **dict(zip(kw, rest)))
+
+        inputs = (x, t_buf, ctx, *kw.values())
+        if not graphed:
+            return x, t_buf, lambda: forward(*inputs)
+        g = self._graphs.get(key, inputs, forward)
+        for dst, src in zip(g.inputs, inputs):
+            if dst is not src:      # a cached graph's k / v were projected in place above
+                dst.copy_(src)
+
+        def replay():
+            g.replay()
+            self.replayed_launches += g.launches
+            return g.outputs
+        return g.inputs[0], g.inputs[1], replay
+
+    def _denoise(self, latents, cond, timesteps, guidance_scale, callback=None, callback_steps=None):
         """pipelines.py:741-759.  Per step: one CUDA graph replay of the DiT forward, then the fused Euler update, which
         also rewrites the model input.  With CFG the forward runs on cat([x, x]) with cat([cond, uncond]) and the update
-        mixes the two predictions first; without (a guidance-distilled model, or guidance_scale < 0) it runs on x.
-        With an object group of more than one member: _denoise_group."""
-        if object_group is not None and r3g_dist.group_layout(object_group)[1][1:]:
-            return self._denoise_group(latents, cond, timesteps, guidance_scale, object_group)
+        mixes the two predictions first; without (a guidance-distilled model, or guidance_scale < 0) it runs on x."""
         B = latents.shape[0]
-        n = len(timesteps)
-        sig = self.scheduler.step_sigmas()
-        # timestep = t.expand(B).to(fp16) / num_train_timesteps, evaluated in fp16 as the reference does
-        t16 = (timesteps.to(torch.float16) / self.scheduler.config.num_train_timesteps).to(self.device)
-        # torch multiplies the fp16 model output by the 0-dim fp32 (sigma_next - sigma) after casting it to the
-        # result dtype, fp16 (schedulers.py:305)
-        dsig = [float((sig[i + 1] - sig[i]).to(torch.float16)) for i in range(n)]
+        t16, dsig = self._schedule(timesteps)
         x = latents.contiguous()
-        do_cfg = cond["main"].shape[0] == 2 * B
-        x_in = torch.cat([x] * 2) if do_cfg else x.clone()
-        t_buf = torch.full((x_in.shape[0],), 0.5, device=self.device, dtype=torch.float16)  # warm-up t; set per step
-        ctx = {"main": cond["main"].contiguous()}
-        # pipelines.py:733-737: a guidance-distilled model takes the scale as an input, [guidance_scale] * B in fp16
-        guidance = None
-        if _guidance_distilled(self.model):
-            guidance = torch.tensor([guidance_scale] * x_in.shape[0], dtype=torch.float16).to(self.device)
-        gkw = lambda gs: {} if gs is None else {"guidance": gs}  # noqa: E731  (a model without guidance_in takes none)
+        ctx = cond["main"].contiguous()
+        do_cfg = ctx.shape[0] == 2 * B
         # An unconditional context whose rows are all one vector (the zeros of unconditional_embedding) lets the DiT run
         # that sample on one text row (Hunyuan3DDiT.forward: uncond_txt_shared).  Checked once per call: one sync.
         shared = False
         if do_cfg and B == 1:
-            un = ctx["main"][1]
+            un = ctx[1]
             shared = bool(torch.equal(un, un[:1].expand_as(un)))
-        # the context's cross-attention k / v, once per call, outside the step graph (into a buffer the graph owns)
-        proj = _context_kv(self.model)
-        kv = proj(ctx["main"]) if proj is not None else None
-        g = None
-        if self.use_cuda_graph and self.model.taps is None:
-            if kv is not None:
-                g = self._graphs.get((x_in.shape, ctx["main"].shape, shared), (x_in, t_buf, ctx["main"], kv),
-                                     lambda xs, ts, cs, kvs: self.model(xs, ts, {"main": cs}, context_kv=kvs))
-                kv = proj(ctx["main"], out=g.inputs[3])
-            else:
-                g = self._graphs.get((x_in.shape, ctx["main"].shape, shared),
-                                     (x_in, t_buf, ctx["main"]) + ((guidance,) if guidance is not None else ()),
-                                     lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs},
-                                                                            uncond_txt_shared=shared, **gkw(gs)))
-            g.inputs[0].copy_(x_in)
-            g.inputs[2].copy_(ctx["main"])
-            if guidance is not None:
-                g.inputs[3].copy_(guidance)
-                guidance = g.inputs[3]
-            x_in, t_buf = g.inputs[:2]
-        if kv is not None:
-            gkw = lambda gs: {"context_kv": kv}  # noqa: E731
-        for i in range(n):
+        x_in, t_buf, step = self._dit_step(torch.cat([x] * 2) if do_cfg else x.clone(), ctx, shared, guidance_scale)
+        for i in range(len(timesteps)):
             t_buf.copy_(t16[i].expand(x_in.shape[0]))
-            if g is not None:
-                g.replay()
-                self.replayed_launches += g.launches
-                v = g.outputs
-            else:
-                v = self.model(x_in, t_buf, ctx, uncond_txt_shared=shared, **gkw(guidance))
+            v = step()
             report = callback is not None and i % callback_steps == 0
             x_prev = x.clone() if report else None
             ops.cfg_euler_step_(x, v, guidance_scale, dsig[i], x_dup=x_in)
@@ -517,9 +524,7 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
         if B != 1:
             raise ValueError(f"an object group generates one object per call, got a batch of {B}")
         n = len(timesteps)
-        sig = self.scheduler.step_sigmas()
-        t16 = (timesteps.to(torch.float16) / self.scheduler.config.num_train_timesteps).to(self.device)
-        dsig = [float((sig[i + 1] - sig[i]).to(torch.float16)) for i in range(n)]
+        t16, dsig = self._schedule(timesteps)
         do_cfg = cond["main"].shape[0] == 2
         x = latents.contiguous().clone()
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(2 * n)]
@@ -528,43 +533,12 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
             ctx = cond["main"][member:member + 1].contiguous()
             # the unconditional sample runs on one text row when all its rows are one vector (see _denoise)
             shared = bool(do_cfg and member == 1 and torch.equal(ctx[0], ctx[0, :1].expand_as(ctx[0])))
-            guidance = None
-            if _guidance_distilled(self.model):
-                guidance = torch.tensor([guidance_scale], dtype=torch.float16).to(self.device)
-            gkw = lambda gs: {} if gs is None else {"guidance": gs}  # noqa: E731
-            t_buf = torch.full((1,), 0.5, device=self.device, dtype=torch.float16)
-            x_in = x
-            proj = _context_kv(self.model)
-            kv = proj(ctx) if proj is not None else None
-            g = None
-            if self.use_cuda_graph and self.model.taps is None:
-                if kv is not None:
-                    g = self._graphs.get((x.shape, ctx.shape, shared), (x, t_buf, ctx, kv),
-                                         lambda xs, ts, cs, kvs: self.model(xs, ts, {"main": cs}, context_kv=kvs))
-                    kv = proj(ctx, out=g.inputs[3])
-                else:
-                    g = self._graphs.get((x.shape, ctx.shape, shared),
-                                         (x, t_buf, ctx) + ((guidance,) if guidance is not None else ()),
-                                         lambda xs, ts, cs, gs=None: self.model(xs, ts, {"main": cs},
-                                                                                uncond_txt_shared=shared, **gkw(gs)))
-                x_in, t_buf = g.inputs[:2]
-                x_in.copy_(x)
-                g.inputs[2].copy_(ctx)
-                if guidance is not None:
-                    g.inputs[3].copy_(guidance)
-                    guidance = g.inputs[3]
-            if kv is not None:
-                gkw = lambda gs: {"context_kv": kv}  # noqa: E731
-            x = x_in            # the Euler update below rewrites the model input in place: no copy per step
+            # the Euler update below rewrites the model input in place: no copy per step
+            x, t_buf, step = self._dit_step(x, ctx, shared, guidance_scale)
             v_pair = torch.empty((2,) + tuple(x.shape[1:]), device=self.device, dtype=x.dtype) if do_cfg else None
             for i in range(n):
                 t_buf.copy_(t16[i].expand(1))
-                if g is not None:
-                    g.replay()
-                    self.replayed_launches += g.launches
-                    v = g.outputs
-                else:
-                    v = self.model(x_in, t_buf, {"main": ctx}, uncond_txt_shared=shared, **gkw(guidance))
+                v = step()
                 if do_cfg:
                     ev[2 * i].record()
                     v = r3g_dist.exchange_cfg_pair(v, v_pair, group)
@@ -613,7 +587,9 @@ class Hunyuan3DDiTFlowMatchingPipeline(Hunyuan3DDiTPipeline):
             if callback is not None:
                 raise NotImplementedError("callback= is not supported with an object group")
             r3g_dist.check_same_inputs(object_group, latents, cond["main"])
-        latents = self._denoise(latents, cond, ts, guidance_scale, callback, callback_steps, object_group=object_group)
+            latents = self._denoise_group(latents, cond, ts, guidance_scale, object_group)
+        else:
+            latents = self._denoise(latents, cond, ts, guidance_scale, callback, callback_steps)
         ev[2].record()
         out = self._export(latents, output_type, box_v, mc_level, num_chunks, octree_resolution, mc_algo,
                            enable_pbar=enable_pbar, object_group=object_group)
