@@ -647,6 +647,15 @@ int validate_linear(r3g_ctx* ctx, const r3g_linear_args* a) {
 constexpr int kRouteWarps = 8;
 constexpr int kMaxExperts = 64;
 
+// Does score a of expert ea rank before score b of expert eb?  Higher first, NaN above every number (torch.topk's
+// order), equal scores and two NaNs to the lower expert.  A strict total order whatever the scores are, so the
+// butterfly below agrees on one winner in every lane, and -1 (no expert, or taken) never beats a valid score or a NaN.
+__device__ __forceinline__ bool route_before(float a, int ea, float b, int eb) {
+  const bool na = a != a, nb = b != b;
+  if (na != nb) return na;
+  return na || a == b ? ea < eb : a > b;
+}
+
 __global__ void __launch_bounds__(32 * kRouteWarps)
 moe_route_kernel(const __half* __restrict__ x, int64_t ldx, const __half* __restrict__ wg, __half* __restrict__ logits,
                  int64_t ldl, int M, int K, int E, int top_k, int cap, int32_t* __restrict__ counts,
@@ -683,14 +692,15 @@ moe_route_kernel(const __half* __restrict__ x, int64_t ldx, const __half* __rest
   float sc[2];
   for (int h = 0; h < 2; ++h) sc[h] = h * 32 + lane < E ? rnd_h(ex[h] * inv) : -1.f;
   for (int j = 0; j < top_k; ++j) {
-    // the highest score, equal scores to the lower expert index
-    float bv = sc[0] >= sc[1] ? sc[0] : sc[1];
-    int be = sc[0] >= sc[1] ? lane : 32 + lane;
+    // the first expert in route_before's order; valid scores are >= 0 or NaN, so the winner is a valid, untaken one
+    const bool hi = route_before(sc[1], 32 + lane, sc[0], lane);
+    float bv = hi ? sc[1] : sc[0];
+    int be = hi ? 32 + lane : lane;
 #pragma unroll
     for (int o = 16; o; o >>= 1) {
       const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
       const int oe = __shfl_xor_sync(0xffffffffu, be, o);
-      if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; }
+      if (route_before(ov, oe, bv, be)) { bv = ov; be = oe; }
     }
     if (lane == (be & 31)) sc[be >> 5] = -1.f;   // taken
     int slot = 0;

@@ -194,7 +194,11 @@ int r3g_mesh_decimate(r3g_ctx* ctx, const float* verts, int64_t nv, const int32_
  *        inside a segment varies between runs), moe_slots[...] = e * moe_cap + p, moe_slot_scale[e * moe_cap + p] =
  *        the score, and x's row is copied to row e * moe_cap + p of moe_slot_x (fp16, K columns, leading dimension
  *        K).  moe_counts (int32 [moe_experts]) is zeroed by the call and ends holding each expert's row count.
- *        moe_cap >= M (an expert takes a row at most once).
+ *        moe_cap >= M (an expert takes a row at most once).  Rows whose logits are not all finite still get moe_top_k
+ *        distinct experts in [0, moe_experts): a NaN score ranks above every number (torch.topk's order), NaNs among
+ *        themselves lower expert first, and a NaN pick's weight is that NaN.  A NaN in x, or a logit that rounds to
+ *        +inf, makes every score of the row NaN, so such a row takes experts 0 .. moe_top_k - 1 with NaN weights; a
+ *        logit of -inf next to a finite one gives its expert score 0.
  *     2 grouped: moe_groups independent GEMMs in one launch, group g = x rows [g * moe_cap, ...) (ldx) against
  *        w[g] (w is [moe_groups, N, K]) plus bias[g] (bias [moe_groups, N] or NULL), written to the same rows of y
  *        (ldy), with act 0 or 2 (erf-GELU) over all columns.  Groups g < moe_experts have moe_counts[g] rows, read on

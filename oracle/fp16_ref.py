@@ -134,19 +134,26 @@ def _act_error(act, h):
     return torch.zeros_like(h)
 
 
-def linear(x, w, bias=None, act=0, act_cols=None, gate=None, gate_rows=1, residual=None, ls_gamma=None,
-           out_f32=False):
-    """r3g_linear on logical rows: x fp16 [M, K], w fp16 [N, K], bias fp16 [N]; act 1 tanh-GELU, 2 erf-GELU, 3 ReLU on
-    columns [act_cols); gate fp16 [B, N] applied to row r with b = r // gate_rows (needs an fp16 residual);
-    residual fp16 [M, N], or float32 [M, N] for the residual_f32 form (then out is float32) with ls_gamma float32 [N].
-    Returns (ref, bound) float64 [M, N]."""
+def _linear_acc(x, w, bias=None):
+    """The fp32 tensor-core acc + bias of r3g_linear (and the MoE modes, which share its operand ring) as an Iv."""
     x64, w64 = x.to(torch.float64), w.to(torch.float64)
     a = x64 @ w64.T
     err = wgmma_sum_bound(x64, w64)
     if bias is not None:
         a = a + bias.to(torch.float64)
         err = err + U24 * (a.abs() + err)
-    v = Iv(a, err)
+    return Iv(a, err)
+
+
+def linear(x, w, bias=None, act=0, act_cols=None, gate=None, gate_rows=1, residual=None, ls_gamma=None,
+           out_f32=False, row_scale=None):
+    """r3g_linear on logical rows: x fp16 [M, K], w fp16 [N, K], bias fp16 [N]; act 1 tanh-GELU, 2 erf-GELU, 3 ReLU on
+    columns [act_cols); gate fp16 [B, N] applied to row r with b = r // gate_rows (needs an fp16 residual);
+    residual fp16 [M, N], or float32 [M, N] for the residual_f32 form (then out is float32) with ls_gamma float32 [N];
+    row_scale fp16 [M], the grouped MoE mode's fp16(fp16(.) * row_scale[r]) (no residual).
+    Returns (ref, bound) float64 [M, N]."""
+    v = _linear_acc(x, w, bias)
+    a = v.mid
     N = w.shape[0]
     if act:
         c0, c1 = act_cols if act_cols is not None else (0, N)
@@ -159,6 +166,8 @@ def linear(x, w, bias=None, act=0, act_cols=None, gate=None, gate_rows=1, residu
             h = v.round16()
             av = h.map(fn).widen(torch.maximum(_act_error(act, h.lo), _act_error(act, h.hi)))
         v = Iv(torch.where(cols, av.mid, v.mid), lo=torch.where(cols, av.lo, v.lo), hi=torch.where(cols, av.hi, v.hi))
+    if row_scale is not None:    # the product of two fp16 values is exact in fp32: one more fp16 rounding
+        return v.round16().scale(row_scale.to(torch.float64)[:, None]).round16().bound()
     if residual is not None and residual.dtype == torch.float32:
         g = ls_gamma.to(torch.float64) if ls_gamma is not None else torch.ones(N, dtype=torch.float64, device=a.device)
         t = v.round16().scale(g)
@@ -175,6 +184,55 @@ def linear(x, w, bias=None, act=0, act_cols=None, gate=None, gate_rows=1, residu
     if out_f32:
         return v.bound()
     return v.round16().bound()
+
+
+# ------------------------------------------------------------------------------------------ r3g_linear moe_mode 1, 3
+EXPF = 2.0 ** -22         # expf (the library is built without fast math): the CUDA maximum of 2 ulp, relative
+
+
+def moe_logits(x, wg):
+    """The route's logits fp16(x wg^T), x fp16 [M, K], wg fp16 [E, K]: lane l of a row's warp runs one fmaf chain over
+    its 8 ceil(K / 256) products (columns 8 l + 256 i + j), then 5 shuffle levels add the lanes' sums in fp32, so any
+    product goes through at most 8 ceil(K / 256) + 5 roundings.  Returns (ref, bound) float64 [M, E]."""
+    x64, w64 = x.to(torch.float64), wg.to(torch.float64)
+    n = 8 * -(-x.shape[1] // 256) + 5
+    gamma = n * U24 / (1 - n * U24)
+    return Iv(x64 @ w64.T, gamma * (x64.abs() @ w64.abs().T)).round16().bound()
+
+
+def moe_scores(logits):
+    """The route's scores fp16(softmax) evaluated in fp32 on the kernel's own fp16 logits [M, E]: the max is exact,
+    lg - mx is one fp32 subtraction (relative error 2^-24, which moves expf's result by expm1(2^-24 |lg - mx|)), expf
+    errs by EXPF relative (and 2^-148 among fp32 subnormals), the sum of the E exponentials goes through 6 fp32
+    additions (one per lane, 5 shuffle levels), and 1 / sum and the product round once each (IEEE).  Returns an Iv float64
+    [M, E]: mid the fp16 of the exact softmax, [lo, hi] the fp16 values a correct kernel may store."""
+    lg = logits.to(torch.float64)
+    d = lg - lg.amax(dim=1, keepdim=True)
+    e = torch.exp(d)
+    p = e / e.sum(dim=1, keepdim=True)
+    sub = torch.where(torch.isinf(d), torch.zeros_like(d), torch.expm1(U24 * d.abs()))   # expf(-inf) = 0 exactly
+    eps = (1 + EXPF) * (1 + sub) - 1                                  # relative error of each exponential
+    g6 = 6 * U24 / (1 - 6 * U24)
+    s_lo = (e * (1 - eps)).sum(dim=1, keepdim=True) * (1 - g6)        # the fp32 sum of the kernel's exponentials
+    s_hi = (e * (1 + eps)).sum(dim=1, keepdim=True) * (1 + g6)
+    hi = e * (1 + eps) * (1 + U24) ** 2 / s_lo + 2.0 ** -146         # 2^-146: subnormal expf and product
+    lo = e * (1 - eps) * (1 - U24) ** 2 / s_hi - 2.0 ** -146
+    return Iv(p, lo=lo.clamp_min(0.0), hi=hi).round16()
+
+
+def moe_combine(x, w, bias, slot_y, ids, slots, residual):
+    """The combine mode: fp16(residual + fp16(routed + fp16(x w^T + bias))), routed the fp16 sum, from 0 in increasing
+    expert order, of rows slots[r, j] of slot_y (x fp16 [M, K], w [N, K], bias [N], slot_y [*, N], ids / slots [M, k],
+    residual [M, N]).  The sum of two fp16 values is exact in float64, and its fp32 rounding rounds to the same fp16, so
+    routed and the two outer roundings are reproduced exactly; only acc + bias carries linear's interval.
+    Returns (ref, bound) float64 [M, N]."""
+    src = slots.long().gather(1, ids.long().argsort(dim=1))
+    y = slot_y.to(torch.float64)
+    routed = torch.zeros(ids.shape[0], y.shape[1], dtype=torch.float64, device=y.device)
+    for j in range(src.shape[1]):
+        routed = f16(routed + y[src[:, j]])
+    v = _linear_acc(x, w, bias).round16().add(routed).round16()
+    return v.add(residual.to(torch.float64)).round16().bound()
 
 
 # ----------------------------------------------------------------------------------------------------- r3g_attention

@@ -86,6 +86,110 @@ def test_linear_mirror_follows_the_documented_dtype_flow():
     R.check_bound(r32 + gam * F.linear(x.float(), w.float(), b.float()).half().float(), ref, bound, "fp32 residual")
 
 
+def test_linear_mirror_row_scale():
+    M, N, K = 37, 64, 40
+    x, w, b = _h(M, K, seed=1), _h(N, K, std=K ** -0.5, seed=2), _h(N, seed=3)
+    s = torch.rand(M, generator=torch.Generator().manual_seed(4)).half()
+    lin = x.double() @ w.double().T + b.double()
+    for act, fn in ((0, lambda t: t), (2, F.gelu)):
+        ref, bound = R.linear(x, w, b, act=act, row_scale=s)
+        assert torch.equal(ref, f16(f16(fn(f16(lin))) * s.double()[:, None]))
+        y = fn(F.linear(x.float(), w.float(), b.float()).half().float()).half()
+        R.check_bound(y * s[:, None], ref, bound, f"row-scaled act={act}")
+
+
+# ------------------------------------------------------------------------------------------------- MoE route / combine
+def _route_logits_like_the_kernel(x, wg):
+    """moe_route_kernel's logits in float32 torch: lane l adds its products x[8 l + 256 i + j] w[...] in (i, j) order
+    (the products of fp16 values are exact, so fmaf is one rounded addition), then the xor-butterfly warp sum."""
+    M, K = x.shape
+    p = x.float()[:, None, :] * wg.float()[None, :, :]                 # [M, E, K], exact
+    lanes = torch.zeros(M, wg.shape[0], 32)
+    for k0 in range(0, K, 256):
+        for j in range(8):
+            cols = torch.arange(32) * 8 + k0 + j
+            ok = cols < K
+            lanes[..., ok] = lanes[..., ok] + p[..., cols[ok]]
+    for o in (16, 8, 4, 2, 1):
+        lanes = lanes + lanes[..., torch.arange(32) ^ o]
+    return lanes[..., 0].half()
+
+
+@pytest.mark.parametrize("K", [8, 1000, 1024])
+def test_moe_logits_mirror(K):
+    x, wg = _h(40, K, seed=K), _h(33, K, std=K ** -0.5, seed=K + 1)
+    ref, bound = R.moe_logits(x, wg)
+    assert torch.equal(ref, f16(x.double() @ wg.double().T))
+    n = 8 * -(-K // 256) + 5
+    assert (bound <= R.ulp16(ref) + 2 * n * 2.0 ** -24 * (x.double().abs() @ wg.double().abs().T)).all()
+    R.check_bound(_route_logits_like_the_kernel(x, wg), ref, bound, f"kernel-order fp32 logits K={K}")
+    R.check_bound((x.float() @ wg.float().T).half(), ref, bound, f"torch fp32 logits K={K}")
+
+
+def _route_scores_like_the_kernel(logits):
+    """moe_route_kernel's softmax in float32 torch: per-lane pairs (e, e + 32) added first, then the xor butterfly."""
+    lg = logits.float()
+    M, E = lg.shape
+    ex = torch.exp(lg - lg.amax(dim=1, keepdim=True))
+    pad = torch.zeros(M, 64)
+    pad[:, :E] = ex
+    s = pad[:, :32] + pad[:, 32:]
+    for o in (16, 8, 4, 2, 1):
+        s = s + s[:, torch.arange(32) ^ o]
+    return (ex * (1.0 / s[:, :1])).half()
+
+
+def test_moe_scores_mirror():
+    g = torch.Generator().manual_seed(5)
+    lg = (torch.randn(400, 40, generator=g) * torch.rand(400, 1, generator=g) * 12).half()
+    lg[0] = 0.0                                     # every score equal
+    lg[1, 7] = 60.0                                 # the others underflow to fp16 0
+    lg[2, :5] = -float("inf")                       # a logit of -inf: score 0
+    lg[3, 3] = 65504.0
+    lg[3, 4] = -65504.0                             # lg - mx is inexact in fp32
+    sc = R.moe_scores(lg)
+    p = torch.softmax(lg.double(), dim=1)
+    assert torch.equal(sc.mid, f16(p))
+    assert (sc.hi - sc.lo <= R.ulp16(sc.mid)).all() and (sc.hi > sc.lo).any()
+    assert torch.equal(sc.mid[0], torch.full((40,), 0.025, dtype=torch.float64).half().double())
+    assert (sc.hi[1, torch.arange(40) != 7] == 0).all() and (sc.lo[1, 7] == 1)
+    assert (sc.hi[2, :5] == 0).all()
+    for what, got in (("torch half softmax", torch.softmax(lg.float(), dim=1).half()),
+                      ("kernel-order fp32 softmax", _route_scores_like_the_kernel(lg))):
+        g64 = got.double()
+        assert ((sc.lo <= g64) & (g64 <= sc.hi)).all(), what
+    # where the k-th and (k+1)-th intervals are apart, the top k of the mirror is torch.topk's
+    for k in (1, 2, 4):
+        order = torch.sort(-sc.mid, dim=1, stable=True).indices
+        kth = sc.lo.gather(1, order[:, k - 1:k])[:, 0]
+        next_hi = sc.hi.gather(1, order[:, k:k + 1])[:, 0]
+        clear = kth > next_hi
+        assert clear.float().mean() > 0.5
+        want = torch.topk(torch.softmax(lg.float(), dim=1), k, dim=1).indices
+        assert torch.equal(order[clear, :k].sort(dim=1).values, want[clear].sort(dim=1).values)
+
+
+def test_moe_combine_mirror_is_sequential_fp16_adds():
+    M, N, K, E, k = 50, 24, 40, 5, 3
+    x, w, b = _h(M, K, seed=1), _h(N, K, std=K ** -0.5, seed=2), _h(N, seed=3)
+    g = torch.Generator().manual_seed(4)
+    ids = torch.stack([torch.randperm(E, generator=g)[:k] for _ in range(M)]).int()
+    cap = M + 3
+    slots = (ids * cap + torch.randint(0, cap, (M, k), generator=g)).int()
+    slot_y = _h(E * cap, N, std=2, seed=5)
+    res = _h(M, N, std=4, seed=6)
+    ref, bound = R.moe_combine(x, w, b, slot_y, ids, slots, res)
+    shared = (x.double() @ w.double().T + b.double()).half()
+    routed = torch.zeros(M, N, dtype=torch.float16)
+    for r in range(M):
+        for j in ids[r].long().argsort():
+            routed[r] = routed[r] + slot_y[slots[r, j]]
+    assert torch.equal(ref, (res + (routed + shared)).double())
+    y32 = F.linear(x.float(), w.float(), b.float()).half()
+    R.check_bound(res + (routed + y32), ref, bound, "fp32 torch shared expert")
+    assert (bound == 0).float().mean() > 0.9 and (bound > 0).any()    # only near an fp16 rounding boundary
+
+
 def test_wgmma_sum_bound_covers_a_truncating_blocked_sum():
     """A k16-blocked fp32 sum that truncates every addend to the block's largest exponent stays inside the bound."""
     x, w = _h(8, 96, seed=1), _h(8, 96, seed=2)

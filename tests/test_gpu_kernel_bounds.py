@@ -1,6 +1,8 @@
-"""GPU: r3g_linear, r3g_attention and the row kernels against the float64 mirrors of oracle/fp16_ref.py, element by
-element within the error bound its analysis gives (check_bound), at the shapes, strides and epilogues where tiles,
-rings and masks change, plus the properties that hold bit for bit."""
+"""GPU: r3g_linear (with its MoE modes), r3g_attention and the row kernels against the float64 mirrors of
+oracle/fp16_ref.py, element by element within the error bound its analysis gives (check_bound), at the shapes, strides
+and epilogues where tiles, rings and masks change, plus the properties that hold bit for bit."""
+
+import itertools
 
 import pytest
 import torch
@@ -395,3 +397,266 @@ def test_points_fourier(path, include_pi, f32):
     check_bound(out, ref, bound, f"points_fourier {path} pi={include_pi} f32={f32}")
     assert (bound <= R.ulp16(ref)).all()
     assert (out[:, 3 + 6 * F:] == 0).all()
+
+
+# ------------------------------------------------------------------------------------------------------ r3g_linear MoE
+GUARD16 = -4320.0     # fp16 guard fill of the MoE output buffers (exact in fp16)
+GUARD32 = -7          # int32 guard fill of ids / slots; counts past E are zero, see _route_bufs
+
+
+def _bits(t):
+    """fp16 as int16, so that NaNs compare by their bits."""
+    return t.view(torch.int16) if t.dtype == torch.float16 else t
+
+
+def _route_bufs(M, E, k, K, cap):
+    """moe_route's output buffers as leading views of larger guard-filled ones.  The larger ones hold one spare
+    segment of cap rows past slot_x / slot_scale's E * cap, 64 spare entries past ids / weights / slots, and 8 zeroed
+    counters past counts: a kernel that routed a row to expert E would count it from 0 and write inside the spare
+    segment, where the guards show it, instead of outside the allocation."""
+    i32 = dict(device=DEV, dtype=torch.int32)
+    h = dict(device=DEV, dtype=torch.float16)
+    big = dict(counts=torch.zeros(E + 8, **i32), ids=torch.full((M * k + 64,), GUARD32, **i32),
+               weights=torch.full((M * k + 64,), GUARD16, **h), slots=torch.full((M * k + 64,), GUARD32, **i32),
+               slot_x=torch.full(((E + 1) * cap, K), GUARD16, **h),
+               slot_scale=torch.full(((E + 1) * cap,), GUARD16, **h))
+    views = dict(counts=big["counts"][:E], ids=big["ids"][:M * k].view(M, k), weights=big["weights"][:M * k].view(M, k),
+                 slots=big["slots"][:M * k].view(M, k), slot_x=big["slot_x"][:E * cap],
+                 slot_scale=big["slot_scale"][:E * cap])
+    return big, views
+
+
+def _route(x, wg, k, cap):
+    """One route launch; the logits go to columns [2, 2 + E) of a guard-filled [M, E + 5] buffer."""
+    M, K = x.shape
+    E = wg.shape[0]
+    big, v = _route_bufs(M, E, k, K, cap)
+    lbuf = torch.full((M, E + 5), GUARD16, device=DEV, dtype=torch.float16)
+    logits = _ops().moe_route(x, wg, top_k=k, cap=cap, out=lbuf[:, 2:2 + E], **v)
+    return logits, lbuf, big, v
+
+
+def _check_route_layout(x, E, k, cap, lbuf, big, v):
+    """What holds whatever the scores: ids in [0, E) and distinct in a row, counts their bincount, slots in the id's
+    segment at positions 0 .. count - 1 (a permutation), the slot rows copies of x with the weights as their scale, and
+    every byte the route must not write still holding its guard."""
+    M, K = x.shape
+    ids, slots = v["ids"].long(), v["slots"].long()
+    assert ((ids >= 0) & (ids < E)).all(), "expert id out of range"
+    assert (ids.sort(dim=1).values.diff(dim=1) > 0).all(), "an expert taken twice in a row"
+    counts = torch.bincount(ids.flatten(), minlength=E)
+    assert torch.equal(v["counts"].long(), counts)
+    assert torch.equal(slots // cap, ids)
+    s = slots.flatten().sort().values
+    start = torch.cumsum(counts, 0) - counts
+    assert torch.equal(s % cap, torch.arange(M * k, device=DEV) - start[s // cap]), "segment positions"
+    assert torch.equal(_bits(v["slot_x"][slots]), _bits(x)[:, None, :].expand(M, k, K))
+    assert torch.equal(_bits(v["slot_scale"][slots]), _bits(v["weights"]))
+    used = torch.zeros((E + 1) * cap, dtype=torch.bool, device=DEV)
+    used[slots.flatten()] = True
+    assert (big["slot_x"] == GUARD16).all(dim=1)[~used].all() and (big["slot_scale"][~used] == GUARD16).all()
+    assert (big["counts"][E:] == 0).all()
+    assert (big["ids"][M * k:] == GUARD32).all() and (big["slots"][M * k:] == GUARD32).all()
+    assert (big["weights"][M * k:] == GUARD16).all()
+    assert (lbuf[:, :2] == GUARD16).all() and (lbuf[:, 2 + E:] == GUARD16).all()
+
+
+def _check_route_picks(logits, v, rows, what):
+    """On `rows`, against the score intervals of the kernel's own logits: every weight in its expert's interval, no
+    chosen interval wholly below an unchosen one, and the picks in the kernel's order (non-increasing weights, equal
+    weights lower expert first)."""
+    sc = R.moe_scores(logits[rows])
+    ids, w = v["ids"][rows].long(), v["weights"][rows].double()
+    assert ((sc.lo.gather(1, ids) <= w) & (w <= sc.hi.gather(1, ids))).all(), f"{what}: weight outside its interval"
+    chosen = torch.zeros_like(sc.lo, dtype=torch.bool).scatter_(1, ids, True)
+    lowest_chosen = torch.where(chosen, sc.hi, torch.full_like(sc.hi, float("inf"))).amin(dim=1)
+    best_unchosen = torch.where(chosen, torch.full_like(sc.lo, -float("inf")), sc.lo).amax(dim=1)
+    assert (lowest_chosen >= best_unchosen).all(), f"{what}: an expert chosen over a surely higher one"
+    assert (w[:, 1:] <= w[:, :-1]).all(), f"{what}: picks out of order"
+    tie = w[:, 1:] == w[:, :-1]
+    assert (ids[:, 1:] > ids[:, :-1])[tie].all(), f"{what}: equal scores not lower expert first"
+
+
+ROUTE_EK = [(1, 1), (8, 2), (4, 4), (33, 3), (64, 4)]
+
+
+@pytest.mark.parametrize("layout", ["cap_M", "cap_M37_strided_x"])
+@pytest.mark.parametrize("M", [1, 7, 8884])
+@pytest.mark.parametrize("K", [8, 1000, 1024])
+@pytest.mark.parametrize("E,k", ROUTE_EK)
+def test_moe_route(E, k, K, M, layout):
+    """E = 64 fills both score registers of every lane, E = 33 one lane's second register, E = 1 leaves 31 lanes idle;
+    K = 8 and 1000 leave lanes idle in the last 256-column pass of the gate dot products."""
+    seed = E * 7 + K + M
+    strided = layout != "cap_M"
+    cap = M + 37 if strided else M
+    x = _randn(M, K + 24, seed=seed)[:, 8:8 + K] if strided else _randn(M, K, seed=seed)
+    wg = _randn(E, K, std=2 * K ** -0.5, seed=seed + 1)
+    logits, lbuf, big, v = _route(x, wg, k, cap)
+    what = f"route E={E} k={k} K={K} M={M} {layout}"
+    check_bound(logits, *R.moe_logits(x, wg), what + " logits")
+    _check_route_picks(logits, v, slice(None), what)
+    _check_route_layout(x, E, k, cap, lbuf, big, v)
+
+
+@pytest.mark.parametrize("k", [1, 2, 3, 4])
+def test_moe_route_ties_go_to_the_lower_expert(k):
+    """Three pairs of identical gate rows, which dominate the others: across lanes (0 / 1), across one lane's two
+    registers (3 / 35) and across the register boundary (31 / 32).  Their logits are bit-identical, so is every score;
+    the lower expert of a pair comes first, and an odd k takes the lower one alone."""
+    E, K, M = 64, 1000, 3000
+    x = _randn(M, K, seed=k)
+    wg = _randn(E, K, std=0.1 * K ** -0.5, seed=k + 1)
+    strong = _randn(3, K, std=3 * K ** -0.5, seed=k + 2)
+    pairs = [(0, 1), (3, 35), (31, 32)]
+    for i, (a, b) in enumerate(pairs):
+        wg[a] = strong[i]
+        wg[b] = strong[i]
+    logits, lbuf, big, v = _route(x, wg, k, M)
+    check_bound(logits, *R.moe_logits(x, wg), f"ties k={k} logits")
+    _check_route_picks(logits, v, slice(None), f"ties k={k}")
+    _check_route_layout(x, E, k, M, lbuf, big, v)
+    ids = v["ids"].long()
+
+    def pos(e):     # expert e's pick position in each row, k where it is not picked
+        hit = ids == e
+        return torch.where(hit.any(dim=1), hit.int().argmax(dim=1), torch.full_like(ids[:, 0], k))
+    for a, b in pairs:
+        assert torch.equal(_bits(logits[:, a]), _bits(logits[:, b]))
+        pa, pb = pos(a), pos(b)
+        assert (pa < k).any(), (a, b)          # the pair is chosen on some rows
+        assert (pa < pb)[pb < k].all(), f"expert {b} taken before or without its twin {a}"
+
+
+@pytest.mark.parametrize("kind", ["all_equal", "underflow"])
+@pytest.mark.parametrize("E,k", ROUTE_EK)
+def test_moe_route_exact_orders(E, k, kind):
+    """all_equal: one gate row for every expert, so every score ties: ids 0 .. k-1.  underflow: expert `hot` leads by
+    about 64, every other score rounds to fp16 0 (and ties at 0): hot, then the lowest other experts."""
+    M, K = 777, 1000
+    hot = E - 1 - E // 3
+    x = _randn(M, K, seed=E + k)
+    if kind == "all_equal":
+        wg = _randn(1, K, std=K ** -0.5, seed=E).expand(E, K).contiguous()
+        want = list(range(k))
+    else:
+        x[:, :8] = 4.0
+        wg = _randn(E, K, std=K ** -0.5, seed=E)
+        wg[:, :8] = 0.0
+        wg[hot, :8] = 2.0
+        want = [hot] + [e for e in range(E) if e != hot][:k - 1]
+    logits, lbuf, big, v = _route(x, wg, k, M)
+    check_bound(logits, *R.moe_logits(x, wg), f"{kind} E={E} k={k} logits")
+    _check_route_picks(logits, v, slice(None), f"{kind} E={E} k={k}")
+    _check_route_layout(x, E, k, M, lbuf, big, v)
+    assert torch.equal(v["ids"].long(), torch.tensor(want, device=DEV).expand(M, k))
+    if kind == "underflow" and k > 1:
+        assert (v["weights"][:, 1:] == 0).all() and (v["weights"][:, 0] == 1).all()
+
+
+@pytest.mark.parametrize("E,k", [(1, 1), (8, 2), (33, 3), (64, 4)])
+def test_moe_route_nonfinite_rows(E, k):
+    """Rows with a NaN in x (in the first and in the last 256-column pass), a logit that rounds to +inf and one that
+    rounds to -inf, among finite rows of one launch.  The NaN and +inf rows have only NaN scores: experts 0 .. k-1 with
+    NaN weights (NaN ranks above every number, lower expert first).  The -inf expert's score is 0 (for E = 1 every
+    logit is -inf and the row is a NaN row).  The finite rows route as in a launch without the others.  Every output is
+    a leading view of a guard-filled buffer sized so that a route to expert E stays inside it and shows."""
+    M, K = 300, 1000
+    cap = M + 37
+    hot = E // 2
+    x = _randn(M, K, seed=E)
+    x[:, :8] = 0.0
+    wg = _randn(E, K, std=2 * K ** -0.5, seed=E + 1)
+    wg[hot, :8] = 1000.0
+    x[5, 3] = float("nan")
+    x[150, 999] = float("nan")
+    x[77, :8] = 10.0                 # logit of `hot` 80000 -> +inf
+    x[231, :8] = -10.0               # -80000 -> -inf
+    bad = [5, 77, 150, 231]
+    logits, lbuf, big, v = _route(x, wg, k, cap)
+    _check_route_layout(x, E, k, cap, lbuf, big, v)
+    assert torch.isnan(logits[[5, 150]]).all()
+    assert logits[77, hot] == float("inf") and logits[231, hot] == -float("inf")
+    good = torch.ones(M, dtype=torch.bool, device=DEV)
+    good[bad] = False
+    ref, bound = R.moe_logits(x[good], wg)
+    check_bound(logits[good], ref, bound, f"nonfinite E={E} logits of the finite rows")
+    nan_rows = [5, 77, 150] + ([231] if E == 1 else [])
+    for r in nan_rows:
+        assert torch.equal(v["ids"][r].long(), torch.arange(k, device=DEV)), (r, v["ids"][r])
+        assert torch.isnan(v["weights"][r]).all(), r
+    scored = good.clone()
+    if E > 1:
+        scored[231] = True
+        assert (v["weights"][231][v["ids"][231] == hot] == 0).all()
+    _check_route_picks(logits, v, scored, f"nonfinite E={E} k={k}")
+    _, _, _, alone = _route(x[good], wg, k, cap)
+    assert torch.equal(v["ids"][good], alone["ids"]) and torch.equal(v["weights"][good], alone["weights"])
+
+
+def _combine_layout(M, E, k, cap, seed):
+    """ids [M, k]: k distinct experts per row, in every order for k = 3 and in 8 of the 24 for k = 4, row by row; slots
+    into a cap-row segment per expert, at a random permutation of positions 0 .. count - 1 within each segment."""
+    g = torch.Generator().manual_seed(seed)
+    chosen = torch.rand(M, E, generator=g).argsort(dim=1)[:, :k].sort(dim=1).values
+    orders = list(itertools.permutations(range(k)))
+    if k == 4:
+        orders = orders[::3]
+    order = torch.tensor(orders)[torch.arange(M) % len(orders)]
+    ids = chosen.gather(1, order)
+    flat = ids.flatten()
+    by_seg = (flat * (M * k) + torch.randperm(M * k, generator=g)).argsort()
+    counts = torch.bincount(flat, minlength=E)
+    start = torch.cumsum(counts, 0) - counts
+    pos = torch.empty_like(flat)
+    pos[by_seg] = torch.arange(M * k) - start[flat[by_seg]]
+    return ids, (ids * cap + pos.view(M, k)), counts
+
+
+@pytest.mark.parametrize("alias", [True, False])
+@pytest.mark.parametrize("M", [1, 129, 8884])
+@pytest.mark.parametrize("N", [8, 136, 392])
+@pytest.mark.parametrize("k", [1, 2, 3, 4])
+def test_moe_combine(k, N, M, alias):
+    """The combine mode against its mirror: out (and the residual, when it is not out) a view into a wider buffer, the
+    routed rows of slot_y in cap = M + 37 segments whose unused rows are NaN; N = 136 and 392 end in partial column
+    tiles.  Moving rows inside each segment of slot_y, with slots moved to match, gives the same bits."""
+    ops = _ops()
+    E, K = 6, 256
+    cap = M + 37
+    seed = k * 1000 + N + M
+    ids, slots, counts = _combine_layout(M, E, k, cap, seed)
+    ids, slots = ids.int().to(DEV), slots.int().to(DEV)
+    slot_y = torch.full((E * cap, N), float("nan"), device=DEV, dtype=torch.float16)
+    used = slots.long().flatten()
+    slot_y[used] = _randn(used.numel(), N, std=0.7, seed=seed + 1)
+    x, w, b = _randn(M, K, seed=seed + 2), _randn(N, K, std=K ** -0.5, seed=seed + 3), _randn(N, seed=seed + 4)
+    res = _randn(M, N, std=2.0, seed=seed + 5)
+    ref, bound = R.moe_combine(x, w, b, slot_y, ids, slots, res)
+
+    def run(slot_y, slots):
+        obuf = torch.full((M, N + 24), GUARD16, device=DEV, dtype=torch.float16)
+        out = obuf[:, 8:8 + N]
+        if alias:
+            out.copy_(res)
+            residual = out
+        else:
+            rbuf = torch.full_like(obuf, GUARD16)
+            residual = rbuf[:, 8:8 + N]
+            residual.copy_(res)
+        ops.moe_combine(x, w, b, slot_y=slot_y, ids=ids, slots=slots, residual=residual, out=out)
+        outside = torch.ones_like(obuf, dtype=torch.bool)
+        outside[:, 8:8 + N] = False
+        assert (obuf[outside] == GUARD16).all()
+        if not alias:
+            assert torch.equal(residual, res)
+        return out
+
+    out = run(slot_y, slots)
+    check_bound(out, ref, bound, f"combine k={k} N={N} M={M} alias={alias}")
+    # reverse the rows of every segment: position p of expert e moves to count_e - 1 - p
+    e, p = slots.long() // cap, slots.long() % cap
+    moved = e * cap + counts.to(DEV)[e] - 1 - p
+    slot_y2 = torch.full_like(slot_y, float("nan"))
+    slot_y2[moved.flatten()] = slot_y[slots.long().flatten()]
+    assert torch.equal(run(slot_y2, moved.int()), out)

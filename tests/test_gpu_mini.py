@@ -1,6 +1,7 @@
-"""GPU: the Hunyuan3D-2mini denoiser (HunYuanDiTPlain) on r3g -- MoE routing, the grouped expert GEMM and the combine
-epilogue (r3g_linear moe_mode), the whole DiT against the float32 oracle (oracle/hy3d_mini_ref.py) on the routing the
-kernels chose, CUDA-graph replay, and image -> mesh with the 2mini configuration."""
+"""GPU: the Hunyuan3D-2mini denoiser (HunYuanDiTPlain) on r3g -- the grouped expert GEMM (r3g_linear moe_mode; the
+route and combine modes are checked in test_gpu_kernel_bounds.py), the whole DiT against the float32 oracle
+(oracle/hy3d_mini_ref.py) on the routing the kernels chose, CUDA-graph replay, and image -> mesh with the 2mini
+configuration."""
 import os
 import sys
 
@@ -19,83 +20,58 @@ def _ops():
     return ops
 
 
-def _route(x, wg, k):
-    ops = _ops()
-    M, K = x.shape
-    E = wg.shape[0]
-    d = x.device
-    bufs = dict(slot_x=torch.empty(E * M, K, device=d, dtype=torch.float16),
-                slot_scale=torch.empty(E * M, device=d, dtype=torch.float16),
-                counts=torch.empty(E, device=d, dtype=torch.int32), ids=torch.empty(M, k, device=d, dtype=torch.int32),
-                weights=torch.empty(M, k, device=d, dtype=torch.float16),
-                slots=torch.empty(M, k, device=d, dtype=torch.int32))
-    logits = ops.moe_route(x, wg, top_k=k, cap=M, **bufs)
-    return logits, bufs
+GROUPED_COUNTS = {"uniform": [300, 300, 300, 300], "one_expert": [300, 0, 0, 0], "empty_expert": [129, 0, 257, 64],
+                  "one_row": [1, 1, 0, 1], "ragged": [127, 131, 200, 5]}
 
 
-@pytest.mark.parametrize("E", [8, 5, 40])
-def test_route_matches_a_float64_gate(E):
-    """E = 40 puts experts in both of a lane's registers; E = 5 leaves most lanes without an expert."""
-    torch.manual_seed(0)
-    M, K, k = 1000, 1024, 2
-    x = torch.randn(M, K, device="cuda").half()
-    wg = (torch.randn(E, K, device="cuda") * 0.05).half()
-    logits, b = _route(x, wg, k)
-    torch.cuda.synchronize()
-    s64 = torch.softmax(x.double() @ wg.double().t(), -1)
-    top = torch.sort(s64, -1, descending=True)
-    clear = (top.values[:, k - 1] - top.values[:, k]) > 2e-3     # the k-th and (k+1)-th scores differ
-    assert clear.float().mean() > 0.5
-    got = torch.sort(b["ids"].long(), -1).values
-    want = torch.sort(top.indices[:, :k], -1).values
-    assert torch.equal(got[clear], want[clear])
-    # weights: the softmax of the kernel's fp16 logits within 1 fp16 ulp of float64; no expert past E is chosen
-    w64 = torch.gather(torch.softmax(logits.double(), -1), 1, b["ids"].long())
-    ulp = 2.0 ** (torch.floor(torch.log2(w64)) - 10)
-    assert ((b["weights"].double() - w64).abs() <= ulp).all()
-    assert int(b["ids"].max()) < E and int(b["ids"].min()) >= 0
-    # every (row, k) sits in its expert's segment, each row once per expert, and the copies are the rows
-    assert int(b["counts"].sum()) == M * k
-    slots = b["slots"].long()
-    assert torch.equal(slots // M, b["ids"].long())
-    assert len(torch.unique(slots)) == M * k
-    assert torch.equal(b["slot_x"][slots[:, 0]], x) and torch.equal(b["slot_x"][slots[:, 1]], x)
-    assert torch.equal(b["counts"].long(), torch.bincount(b["ids"].long().flatten(), minlength=E))
-    assert torch.equal(b["slot_scale"][slots], b["weights"])
-    # logits: fp16 of an fp32 dot product: within 1 fp16 ulp of float64 plus the fp32 accumulation bound K eps32 |x||w|
-    l64 = x.double() @ wg.double().t()
-    acc = x.shape[1] * 2.0 ** -24 * (x.double().abs() @ wg.double().abs().t())
-    assert ((logits.double() - l64).abs() <= 2.0 ** (torch.floor(torch.log2(l64.abs().clamp_min(2 ** -14))) - 10)
-            + acc).all()
-
-
-@pytest.mark.parametrize("dist", ["uniform", "one_expert", "empty_expert", "one_row", "ragged"])
+@pytest.mark.parametrize("dist", list(GROUPED_COUNTS) + ["no_bias", "no_experts", "strided", "n8", "k200"])
 def test_grouped_gemm_is_per_expert_linear_bit_for_bit(dist):
+    """Each group equals ops.linear of its rows bit for bit, and the fp16_ref mirror, with and without the row scale.
+    The cases past the row distributions take the ragged one and change one thing: no bias; experts = 0 (every group
+    has cap rows); x and out strided views of wider buffers; N = 8 (one partial column tile); K = 200."""
+    import fp16_ref as R
     ops = _ops()
     torch.manual_seed(1)
-    G, E, cap, N, K = 5, 4, 300, 384, 256
-    counts = {"uniform": [300, 300, 300, 300], "one_expert": [300, 0, 0, 0], "empty_expert": [129, 0, 257, 64],
-              "one_row": [1, 1, 0, 1], "ragged": [127, 131, 200, 5]}[dist]
-    x = torch.randn(G * cap, K, device="cuda").half()
+    G, cap = 5, 300
+    E = 0 if dist == "no_experts" else 4
+    N = 8 if dist == "n8" else 384
+    K = 200 if dist == "k200" else 256
+    counts = GROUPED_COUNTS.get(dist, GROUPED_COUNTS["ragged"])
+    strided = dist == "strided"
+    xbuf = torch.randn(G * cap, K + 40, device="cuda").half()
+    x = xbuf[:, 16:16 + K] if strided else xbuf[:, :K].contiguous()
     w = (torch.randn(G, N, K, device="cuda") * 0.05).half()
-    b = (torch.randn(G, N, device="cuda") * 0.1).half()
+    b = None if dist == "no_bias" else (torch.randn(G, N, device="cuda") * 0.1).half()
     scale = torch.rand(G * cap, device="cuda").half()
     cnt = torch.tensor(counts, device="cuda", dtype=torch.int32)
+    # ops.linear takes N % 32 == 0: the reference pads w (and bias) with zero rows and keeps the first N columns
+    Np = -(-N // 32) * 32
+    wp = torch.zeros(G, Np, K, device="cuda", dtype=torch.float16)
+    wp[:, :N] = w
+    bp = None if b is None else torch.zeros(G, Np, device="cuda", dtype=torch.float16)
+    if bp is not None:
+        bp[:, :N] = b
     for act, rs in ((ops.ACT_GELU_ERF, None), (ops.ACT_NONE, scale)):
-        out = torch.full((G * cap, N), float("nan"), device="cuda", dtype=torch.float16)
+        obuf = torch.full((G * cap, N + 24), float("nan"), device="cuda", dtype=torch.float16)
+        out = obuf[:, 8:8 + N] if strided else obuf[:, :N].contiguous()
         ops.moe_grouped(x, w, b, counts=cnt, experts=E, out=out, act=act, row_scale=rs)
         for g in range(G):
             n = counts[g] if g < E else cap
             if n == 0:
                 continue
             rows = slice(g * cap, g * cap + n)
-            ref = ops.linear(x[rows], w[g], b[g], act=act)
+            bg = None if b is None else b[g]
+            ref = ops.linear(x[rows], wp[g], None if bp is None else bp[g], act=act)[:, :N]
             if rs is not None:
                 ref = ref * rs[rows, None]
             assert torch.equal(out[rows], ref), (dist, g, act)
-        # rows past a group's count are not written
+            R.check_bound(out[rows], *R.linear(x[rows], w[g], bg, act=act, row_scale=None if rs is None else rs[rows]),
+                          f"grouped {dist} group {g} act={act} scaled={rs is not None}")
+        # rows past a group's count are not written, nor is anything outside the out view
         for g in range(E):
             assert torch.isnan(out[g * cap + counts[g]:(g + 1) * cap]).all()
+        if strided:
+            assert torch.isnan(obuf[:, :8]).all() and torch.isnan(obuf[:, 8 + N:]).all()
 
 
 def test_moe_block_matches_the_oracle_on_the_kernel_routing():
